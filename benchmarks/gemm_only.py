@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""The layer's three dense products alone (for ncu captures and A/B timing of the tcgen05 3xTF32 GEMMs).
+"""The layer's three dense products alone (for ncu captures and A/B timing of the wgmma 3xTF32 GEMMs).
 
     python benchmarks/gemm_only.py [--rows 10000000] [--n 256] [--k 256] [--steps 5] [--bsplit 0|1] [--mode 0|1]
 """

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Timing of the non-headline BASELINE.json configs on one B200 (parity for these is in tests/;
+"""Timing of the non-headline BASELINE.json configs on one GPU (parity for these is in tests/;
 they are not bench.py lines).  Prints one JSON object per config.
 
   config 2: 3-layer SAGEConv(mean), synthetic power-law 10 M nodes / 100 M edges, h = 256, fp32

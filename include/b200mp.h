@@ -1,11 +1,11 @@
 /*
- * b200mp.h -- C ABI of the B200-native message-passing aggregation engine.
+ * b200mp.h -- C ABI of the H100-native (sm_90a) message-passing aggregation engine.
  *
  * This is the drop-in boundary (SURVEY.md section 8(b), DESIGN.md section 2).  The reference
  * (pyg-team/pytorch_geometric v2.9.0) has no FFI of its own: it late-binds a small set of
  * operator signatures (torch_scatter.*, torch.ops.torch_sparse.spmm_*, pyg_lib.ops.*) and a few
  * Python functions.  Each entry point below states which of those it replaces (file:line under
- * /root/reference/torch_geometric).  INTEGRATION.md shows the reference-side binding.
+ * torch_geometric/ of the reference, v2.9.0).  INTEGRATION.md shows the reference-side binding.
  *
  * Conventions
  *  - plain pointers and sizes; no torch types.  All pointers are DEVICE pointers unless the
@@ -404,14 +404,14 @@ int b200mp_attn_csr_backward(int mode, const void* rowptr, const void* col, cons
                              int val_dtype, void* stream);
 
 /* ------------------------------------------------------------------ dense transform on tensor cores
- * fp32-accurate 3xTF32 GEMMs (tcgen05 + TMEM + TMA, csrc/gemm_tf32x3.cu) for the layer's
+ * fp32-accurate 3xTF32 GEMMs (wgmma + TMA, csrc/gemm_tf32x3.cu) for the layer's
  * Linear (nn/dense/linear.py:121-127: F.linear, run by the reference as strict-fp32 cuBLAS):
  *   b200mp_linear_tf32x3            y [M,N]  = x [M,K] . w[N,K]^T
  *   b200mp_linear_grad_input_tf32x3 gx[M,K]  = g [M,N] . w[N,K]
  *   b200mp_linear_grad_weight_tf32x3 gw[N,K] = g [M,N]^T . x[M,K]   (deterministic split-K)
  * w_hi/w_lo come from b200mp_split_tf32 (w = w_hi + w_lo, w_hi = rn_tf32(w)); w_lo == NULL means w_hi is
  * the UNSPLIT weight and the kernel splits each B tile in shared memory (one L2 read of W per tile instead
- * of two; needs an output width that is a multiple of 128).  All matrices
+ * of two).  All matrices
  * row-major, contiguous, 16-byte aligned.  Shape limits (else B200MP_ERR_UNSUPPORTED and the caller
  * uses a library GEMM): reduction dim % 32 == 0, output width in {64, 128} or a multiple of 256,
  * and for grad_weight N % 128 == 0. */
@@ -425,7 +425,7 @@ int b200mp_linear_grad_weight_tf32x3(const float* g, const float* x, float* gw, 
                                      int64_t k, void* workspace, int64_t workspace_bytes,
                                      void* stream);
 
-/* Pair form of the TS-mode kernel (A operand in tensor memory): two A streams accumulate into ONE TMEM accumulator,
+/* Pair form: two A streams accumulate into ONE accumulator,
  * the epilogue adds a bias and applies ReLU, and the output columns may be split over two matrices:
  *     [c1 | c2] [M, n1+n2] = act( [a1 | a2] [M, k1+k2] . B + bias )
  * b_layout 0: B = w [n1+n2, k1+k2] row-major (y = A w^T: SAGEConv's lin_l(agg) + lin_r(x) with w = [W_l | W_r],

@@ -1,7 +1,7 @@
 """Restatement of the reference's DEFAULT CPU path for GCNConv on a plain [2,E] edge_index, as the
 exact sequence of ATen calls the reference issues (SURVEY.md section 3.1) -- used as the timed CPU
-arm (`bench.py --impl reference`, `cpu_baseline`) because /root/reference does not exist on the
-GPU box.  TEST / BENCH INFRASTRUCTURE ONLY: never imported by pytorch_geometric_b200/.
+arm (`bench.py --impl reference`, `cpu_baseline`) when the reference package is not installed in
+oracle/_ref.  TEST / BENCH INFRASTRUCTURE ONLY: never imported by pytorch_geometric_b200/.
 
   gcn_norm                 nn/conv/gcn_conv.py:95-113   (add_remaining_self_loops loop.py:623-657,
                                                          scatter _scatter.py:68-70)

@@ -1,4 +1,4 @@
-"""pytorch_geometric_b200 -- a B200-native (sm_100a) message-passing aggregation engine that drops
+"""pytorch_geometric_b200 -- an H100-native (sm_90a) message-passing aggregation engine that drops
 in behind PyG's scatter / segment / softmax / spmm / MessagePassing.propagate path.
 
 Layout: csrc/ (CUDA kernels + the C ABI of include/b200mp.h), _lib.py/ops.py (ctypes binding),

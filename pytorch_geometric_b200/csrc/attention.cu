@@ -101,9 +101,9 @@ __device__ __forceinline__ void merge_ms(float m1, float m2, float& M, float& c1
 // ------------------------------------------------------------------------------------------------ forward
 // STAGED (VPL == 1, G >= 8): the row vectors (and GAT's a_src scalars) of iteration t + 1 are in flight as cp.async
 // copies into lane-private shared-memory slots while iteration t is computed -- twice the rows in flight per warp at the
-// same register budget (the sweeps are latency-bound: 58 % long-scoreboard stalls in profiles/r2_attn_v2.summary.csv).
+// same register budget (the sweeps are latency-bound: most stalls wait on the gathered rows).
 // BT = threads per CTA.  32 (one warp = one work item per CTA) for the staged kernels: a 4-warp CTA holds its slots until
-// the longest of its four power-law rows is done (ncu, r2_attn_v3: 35 % achieved of 50 % theoretical occupancy).
+// the longest of its four power-law rows is done, which wastes occupancy.
 // VAR: 0 = rows gathered into registers, 1 = STAGED (cp.async slots), 2 = EDGE (register form + per-edge feature rows a.ee).
 template <typename T, typename I, int G, int VPL, int MODE, int VAR = 0, int BT = kAttnT>
 __global__ void __launch_bounds__(BT, (VPL == 1 ? (VAR == 2 ? 6 : 8) : 5) * (kAttnT / BT))       // <= 64 registers: 32 warps / SM
@@ -194,8 +194,7 @@ attn_fwd_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, AttnArg
             const int d = t & (D - 1);
             if constexpr (MODE == ATTN_GAT) {
                 // GAT scores need no feature data: take the stage's UNR logits first, move the running max ONCE and rescale
-                // the accumulators once per stage instead of once per edge (the sweep is issue-bound after the staging:
-                // 77 % of the issue slots busy in profiles/r2_attn_v3.summary.csv)
+                // the accumulators once per stage instead of once per edge (the sweep is issue-bound after the staging)
                 float lg[UNR];
                 float mb = m[0];
                 bool any = false;

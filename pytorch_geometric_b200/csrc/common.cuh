@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the b200mp kernels (sm_100a only).
+// common.cuh -- shared helpers for the b200mp kernels (sm_90a only).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -33,7 +33,7 @@ void set_error(const char* fmt, ...);
 
 #define B200MP_LAUNCH_CHECK() B200MP_CUDA(cudaGetLastError())
 
-constexpr int kSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kSMs = 132;  // H100 SXM (fallback only: the device attribute is queried first)
 
 inline int num_sms() {
     static int n = 0;

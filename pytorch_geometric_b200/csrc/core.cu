@@ -44,14 +44,6 @@ extern "C" int b200mp_device_info(int* sm_count, int* cc_major, int* cc_minor, i
 namespace b200mp {
 static int g_spmm_impl = 0;
 int get_option_spmm_impl() { return g_spmm_impl; }
-static int g_gemm_bk = 32;
-int get_option_gemm_bk() { return g_gemm_bk; }
-static int g_gemm_prefetch = 0;
-int get_option_gemm_prefetch() { return g_gemm_prefetch; }
-static int g_gemm_debug = 0;
-int get_option_gemm_debug() { return g_gemm_debug; }
-static int g_gemm_mode = 1;   // TS mode (A operand in TMEM) measured 25 % faster than SS (profiles/r1_summary.md)
-int get_option_gemm_mode() { return g_gemm_mode; }
 static int g_spmm_tune = 0;
 int get_option_spmm_tune() { return g_spmm_tune; }
 static int g_attn_staged = 2;   // cp.async-staged attention sweeps (csrc/attention.cu): 2 = with one-warp CTAs, 1 = 4-warp CTAs, 0 = register-staged loop
@@ -108,25 +100,12 @@ extern "C" int b200mp_set_option(const char* name, int value) {
         b200mp::g_attn_staged = value;
         return B200MP_OK;
     }
-    if (strcmp(name, "gemm_prefetch") == 0) {
-        if (value < 0 || value > 64) return B200MP_ERR_INVALID_ARG;
-        b200mp::g_gemm_prefetch = value;
-        return B200MP_OK;
-    }
-    if (strcmp(name, "gemm_debug") == 0) {
-        b200mp::g_gemm_debug = value;
-        return B200MP_OK;
-    }
-    if (strcmp(name, "gemm_mode") == 0) {
-        if (value != 0 && value != 1) return B200MP_ERR_INVALID_ARG;
-        b200mp::g_gemm_mode = value;
-        return B200MP_OK;
-    }
-    if (strcmp(name, "gemm_bk") == 0) {
-        if (value != 16 && value != 32) return B200MP_ERR_INVALID_ARG;
-        b200mp::g_gemm_bk = value;
-        return B200MP_OK;
-    }
+    // GEMM knobs: validated and accepted so that existing callers keep working, but the sm_90a wgmma GEMM
+    // (csrc/gemm_tf32x3.cu) has one configuration, so they do not change what runs
+    if (strcmp(name, "gemm_prefetch") == 0) return (value < 0 || value > 64) ? B200MP_ERR_INVALID_ARG : B200MP_OK;
+    if (strcmp(name, "gemm_debug") == 0) return B200MP_OK;
+    if (strcmp(name, "gemm_mode") == 0) return (value != 0 && value != 1) ? B200MP_ERR_INVALID_ARG : B200MP_OK;
+    if (strcmp(name, "gemm_bk") == 0) return (value != 16 && value != 32) ? B200MP_ERR_INVALID_ARG : B200MP_OK;
     b200mp::set_error("unknown option %s", name);
     return B200MP_ERR_INVALID_ARG;
 }

@@ -1,7 +1,7 @@
 // csr_dispatch.cuh -- picks the kernel variant for one gather/segment reduce call.
 //   wide rows  (512 B <= row_bytes <= 2 KB, 16 B aligned): persistent TMA-fed streaming kernel
 //   otherwise : lane-group-per-row kernel (csr_reduce.cuh), scalar fallback for odd widths
-// b200mp_set_option("spmm_impl", 1) forces the lane-group kernel (A/B measurements, profiles/).
+// b200mp_set_option("spmm_impl", 1) forces the lane-group kernel (A/B measurements).
 #pragma once
 
 #include "csr_reduce.cuh"
@@ -19,10 +19,8 @@ int csr_reduce_variant(const I* rowptr, const I* col, const float* val, const T*
     const size_t row_bytes = static_cast<size_t>(feat) * sizeof(T);
     const bool tma_ok = row_bytes % 16 == 0 && row_bytes >= 512 && row_bytes <= 2048 && aligned16(x) &&
                         aligned16(out) && (plan.n_chunks == 0 || aligned16(plan.partials));
-    // Measured on B200 (profiles/r1_spmm_tuning.md): the lane-group kernel at 48 warps/SM reaches
-    // 7.1 TB/s of algorithmic bytes on the headline shape, the TMA-fed kernel 3.5 TB/s (it is
-    // issue-bound at 6 warps/SM) -- so "auto" is the lane-group kernel; the TMA variant stays
-    // selectable for the A/B evidence and further tuning.
+    // "auto" is the lane-group kernel: at 48 warps/SM it keeps more rows in flight than the TMA-fed
+    // kernel, which is issue-bound at 6 warps/SM.  The TMA variant stays selectable for A/B timing.
     const int impl = get_option_spmm_impl();
     if (tma_ok && impl == 2 && !plan.accumulate && !plan.peers)
         return csr_tma_launch<T, I, RED, GATHER>(rowptr, col, val, x, out, n_rows, feat, is_mean, inf_to_zero, plan,

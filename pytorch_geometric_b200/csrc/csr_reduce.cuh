@@ -103,7 +103,7 @@ __device__ __forceinline__ float finalize(float acc, int64_t deg, bool is_mean, 
 }
 
 // UNR_OVR / BLOCK / MINB are tuning knobs (independent row loads in flight per lane, CTA size,
-// minimum resident CTAs per SM => register cap); the defaults are the measured best (profiles/).
+// minimum resident CTAs per SM => register cap); defaults below.
 template <typename T, typename I, int G, int VPL, int RED, bool GATHER, int UNR_OVR = 0, int BLOCK = 256,
           int MINB = 1>
 __global__ void __launch_bounds__(BLOCK, MINB)
@@ -340,15 +340,13 @@ inline void launch_vec(const I* rowptr, const I* col, const float* val, const T*
     if (G == 32 && VPL == 2 && RED == B200MP_SUM && GATHER) {
         // the headline shape (F = 256 fp32 / 512 bf16): tuning variants selectable at run time
         switch (get_option_spmm_tune()) {
-            // (the full 11-point sweep and its numbers are in profiles/r1_spmm_tuning.md)
             case 1: B200MP_LAUNCH_TUNED(4, 256, 1); return;     // unconstrained registers (86): 16 warps / SM
             case 2: B200MP_LAUNCH_TUNED(4, 256, 4); return;     // <= 64 regs, 32 warps / SM
             case 3: B200MP_LAUNCH_TUNED(1, 256, 8); return;     // <= 32 regs, 64 warps / SM, 2 loads in flight
             default: break;
         }
     }
-    // Default = the measured best of the sweep in profiles/r1_spmm_tuning.md: occupancy beats
-    // per-lane memory parallelism -- 4 sixteen-byte row loads in flight per lane, 128-thread CTAs,
+    // Default: occupancy over per-lane memory parallelism -- 4 sixteen-byte row loads in flight per lane, 128-thread CTAs,
     // registers capped at 40 (fp32) / 64 (bf16: twice the accumulators) => 48 / 32 warps per SM.
     constexpr int kUnr = VPL >= 4 ? 1 : 4 / VPL;
     if (sizeof(T) == 4) B200MP_LAUNCH_TUNED(kUnr, 128, 12);

@@ -1,7 +1,7 @@
 // csr_tma.cuh -- persistent, TMA-fed variant of the gather + segmented-reduce kernel for wide
 // feature rows (row_bytes >= 512 B, i.e. >= 32 sixteen-byte vectors).
 //
-// Why (profiles/r1_v0_spmm.md): with one lane group per CSR row the chain rowptr -> col -> gather
+// Why: with one lane group per CSR row the chain rowptr -> col -> gather
 // is serialised per row (average degree 11) and the bytes in flight per SM are bounded by
 // registers (8 x 16 B per lane).  Here
 //   * one CTA per SM, persistent; every WARP owns a ring of 32 row slots in shared memory and

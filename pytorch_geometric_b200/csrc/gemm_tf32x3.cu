@@ -1,39 +1,40 @@
-// gemm_tf32x3.cu -- fp32-accurate dense transform on the 5th-gen tensor cores (tcgen05 + TMEM + TMA).
+// gemm_tf32x3.cu -- fp32-accurate dense transform on the Hopper tensor cores (wgmma + TMA + mbarrier).
 //
 // The only GEMM-shaped work on the path is the layer's dense transform (SURVEY.md a14):
 //     y  = x  W^T      [M,K] x [N,K]^T        (forward,       nn/dense/linear.py:121-127)
 //     gx = g  W        [M,N] x [N,K]          (grad wrt input)
 //     gW = g^T x       [N,M] x [M,K]          (grad wrt weight, reduction over the M = #nodes rows)
-// The reference runs them as strict-fp32 cuBLAS SIMT kernels (allow_tf32=False); at the headline
-// shape (M = 10 M, N = K = 256) those are 24-32 ms each and dominate the step.  A single-pass TF32
-// GEMM would be 10x faster but only ~1e-3 accurate, so this kernel uses the error-compensated
+// The reference runs them as strict-fp32 cuBLAS SIMT kernels (allow_tf32=False).  A single-pass TF32
+// GEMM would be much faster but only ~1e-3 accurate, so this kernel uses the error-compensated
 // 3xTF32 split:  a = a_hi + a_lo  (a_hi = rn_tf32(a), a_lo = a - a_hi exactly), and
-//     a*b ~= a_hi*b_hi + a_lo*b_hi + a_hi*b_lo      (dropped term a_lo*b_lo ~ 2^-22 |a b|)
-// accumulated in fp32 in TMEM -- fp32-class accuracy at a third of the TF32 tensor rate.
+//     a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi      (dropped term a_lo*b_lo ~ 2^-22 |a b|)
+// accumulated in fp32 registers -- fp32-class accuracy at a third of the TF32 tensor rate.
 //
-// Structure (one persistent CTA per SM, 384 threads, warp-specialised):
-//   warp 0      TMA producer: cp.async.bulk.tensor.2d of the raw fp32 operand tiles, 128B swizzle
-//   warps 4-7   splitter: turn each landed tile into (hi in place, lo in a second buffer) -- a
-//               layout-agnostic element-wise pass, then fence.proxy.async + mbarrier arrive
-//   warp 1      MMA issuer: one thread issues 4 k-steps x 3 products of tcgen05.mma.kind::tf32
-//               (M=128, N=BN, K=8) per 32-wide k-block, commits to the stage's "empty" barrier
-//   warps 8-11  epilogue: tcgen05.ld 32x32b.x32 TMEM -> registers -> 128-bit global stores,
-//               double-buffered accumulators (2 x BN TMEM columns) so it overlaps the next tile
-// Operands may be K-major (row-major [rows, K]) or MN-major (row-major [K, rows]): tcgen05 takes
-// both for TF32, so all three products read x, g and W exactly as they lie in HBM (no transposes).
-// W is split once into (W_hi, W_lo) by a tiny pre-pass; x and g are split in shared memory.
+// Structure (one persistent CTA per SM, 384 threads = three warpgroups, 128 x BN output tiles, BK = 32):
+//   warpgroup 0     TMA producer: one thread streams the raw fp32 A and B tiles into a 3-deep ring of
+//                   shared-memory stages (cp.async.bulk.tensor.2d, mbarrier complete_tx)
+//   warpgroups 1-2  consumers, 64 output rows each.  Per k-block they
+//                   (1) split the B tile into (hi, lo) K-major 128B-swizzled buffers -- wgmma takes TF32
+//                       operands from shared memory only K-major, so an MN-major B is transposed here;
+//                   (2) load their A fragments straight from the raw tile (either major) into registers and
+//                       split them there: A is the register operand of wgmma, never written back;
+//                   (3) issue 4 k-steps x 3 products of wgmma.m64nBNk8.f32.tf32.tf32 into fp32 registers.
+//                   The epilogue adds the bias, applies ReLU and stores the fragments with masked rows.
+// Operands may be K-major (row-major [rows, K]) or MN-major (row-major [K, rows]), so all three products
+// read x, g and W exactly as they lie in HBM (no transposes in global memory).  W may arrive pre-split
+// (W_hi, W_lo from b200mp_split_tf32): its two tiles are then copied, not re-split.
 #include <cuda.h>
 
 #include "common.cuh"
 
 namespace b200mp {
 
-constexpr int kBM = 128;       // UMMA M
-// BK (fp32 elements per k-block) is a template parameter: 32 = one 128-byte swizzle row, 2 smem
-// stages of 96 KB (BN = 256); 16 = 64-byte rows (SWIZZLE_64B for K-major operands), 4 stages of 48 KB.
-constexpr int kAccStages = 2;
-constexpr int kGemmThreads = 384;     // SS kernel: TMA, MMA, 2 idle, splitter (4-7), epilogue (8-11)
-constexpr int kGemmThreadsTs = 512;   // TS kernel: + a second splitter set (warps 12-15)
+constexpr int kBM = 128;             // output rows per CTA tile (two m64 warpgroups)
+constexpr int kBK = 32;              // fp32 elements of K per stage = one 128-byte swizzle row
+constexpr int kStages = 3;
+constexpr int kGemmThreads = 384;
+constexpr int kConsumerThreads = 256;
+constexpr int kMaxSegments = 120;    // grouped form: the tile -> segment table lives in static shared memory
 
 // ---------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ uint32_t s2u(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -64,345 +65,318 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
         "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
         : "memory");
 }
-// TMA prefetch of one box into L2 (no shared memory, no barrier): issued a few k-blocks ahead so the
-// real load finds its data in L2 instead of paying the HBM latency inside a 2..4 deep smem ring.
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int c0, int c1) {
-    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0),
-                 "r"(c1)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// One lane of a fully converged warp (always the same one, so tcgen05.commit tracks the MMAs it issued).
-// The TS kernel's MMA issuer runs its loop WARP-WIDE and only the tcgen05 instructions sit under this
-// predicate: with `if (lane == 0)` around the whole loop the loop state lives in vector registers and the
-// compiler wraps every UTCHMMA (uniform-datapath operands) in an ELECT / BRA.U.ANY waterfall, ~20 SASS
-// instructions per MMA (profiles/r1_gemm_ts.md).  Measured perf-neutral for the TS kernel; the SS kernel got
-// slower with the same change plus a second splitter set (grad_weight 7.7 -> 9.5 ms inside bench.py), so it
-// keeps its single-thread issuer and one splitter set.
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n"
-        ".reg .pred P;\n"
-        "elect.sync _|P, 0xffffffff;\n"
-        "selp.b32 %0, 1, 0, P;\n"
-        "}\n"
-        : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// 256-bit global store (sm_100+): a thread that owns 8 consecutive fp32 of a row writes one complete
-// 32-byte sector per instruction instead of two half-filled ones.
-__device__ __forceinline__ void stg_v8(float* p, const uint32_t* r) {
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]),
-                 "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
+// the 256 consumer threads only (named barrier 1; warpgroup 0 never takes part)
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory"); }
 __device__ __forceinline__ float rn_tf32(float a) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(a));
     return __uint_as_float(r);
 }
-
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout_type [61,64).
-//   K-major operand : SWIZZLE_128B (2): rows of 128 B (32 tf32 along K), 8-row atoms of 1024 B
-//                     (TMA CU_TENSOR_MAP_SWIZZLE_128B); LBO = 16 B (unused), SBO = 1024 B.
-//   MN-major operand: 32-bit MN-major data only exist as SWIZZLE_128B_BASE32B (1): 128-byte rows of
-//                     32 MN elements, 4 k-rows per 512-byte atom, 32-byte swizzle granule
-//                     (TMA CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B); LBO = stride between 32-element
-//                     MN slabs, SBO = 512 B between groups of 4 k-rows.
-//   K-major with BK = 16: SWIZZLE_64B (4): rows of 64 B, 8-row atoms of 512 B.
-template <bool MN, int BK>
-__device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t slab_stride_bytes) {
-    const uint32_t lbo = MN ? slab_stride_bytes : 16u;
-    const uint32_t sbo = MN ? 512u : (BK == 32 ? 1024u : 512u);
-    const uint64_t layout = MN ? 1ull : (BK == 32 ? 2ull : 4ull);
-    return static_cast<uint64_t>((addr & 0x3ffffu) >> 4) | (static_cast<uint64_t>((lbo >> 4) & 0x3fffu) << 16) |
-           (static_cast<uint64_t>((sbo >> 4) & 0x3fffu) << 32) | (1ull << 46) | (layout << 61);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1) [4,6), a/b format TF32 (2)
-// [7,10)/[10,13), a_major [15], b_major [16] (1 = MN-major), N>>3 [17,23), M>>4 [24,29).
-__host__ __device__ constexpr uint32_t instr_desc(int m, int n, bool a_mn, bool b_mn) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(a_mn) << 15) | (static_cast<uint32_t>(b_mn) << 16) |
-           (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
+
+// d[64 x N] (+)= a[64 x 8] (registers, tf32) . b[8 x N] (shared memory, K-major, tf32)
+__device__ __forceinline__ void wgmma_m64n64k8_tf32_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %37, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
+        : "memory");
+}
+__device__ __forceinline__ void wgmma_m64n128k8_tf32_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %69, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
+        : "memory");
+}
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    if constexpr (BN == 64) wgmma_m64n64k8_tf32_rs(d, a, bdesc, scale_d);
+    else wgmma_m64n128k8_tf32_rs(d, a, bdesc, scale_d);
+}
+
+// Shared-memory matrix descriptor of a K-major 128B-swizzled operand (rows of 128 B = 32 tf32 along K,
+// 8-row atoms of 1024 B, as TMA CU_TENSOR_MAP_SWIZZLE_128B writes them): start>>4 [0,14), LBO>>4 [16,30)
+// (unused for swizzled K-major), SBO>>4 [32,46) = 1024 B between 8-row groups, swizzle mode [62,64) = 1 (128B).
+// The k-step j of a 32-wide block starts 32 B further along the swizzle row.
+__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t addr) {
+    return static_cast<uint64_t>((addr & 0x3ffffu) >> 4) | (1ull << 16) | (static_cast<uint64_t>(1024u >> 4) << 32) | (1ull << 62);
+}
+// byte offset of element (row, k) in a [rows x 32] fp32 tile stored K-major with the 128-byte swizzle
+__device__ __forceinline__ uint32_t sw128_offset(int row, int k) {
+    return static_cast<uint32_t>(row * 128 + ((((k >> 2) ^ (row & 7))) << 4) + ((k & 3) << 2));
 }
 
 struct GemmArgs {
-    float* c;             // output [M, ldc] (or split-K partials [splits, M, ldc])
+    float* c;             // output [M, ldc] (or split-K partials [splits, M, ldc]); n-tiles [0, n_tiles_c1)
+    float* c2;            // second output [M, ldc2]: n-tiles [n_tiles_c1, n_tiles_n) (pair form), else unused
+    const float* bias;    // epilogue: + bias[n] over the concatenated output columns (nullable)
     int64_t m;            // rows of the output tile space (A's MN extent)
-    int64_t ldc;
-    int n_tiles_m, n_tiles_n;
+    int64_t ldc, ldc2;
+    int n_tiles_m, n_tiles_n, n_tiles_c1;
     int k_blocks;         // total 32-wide k-blocks
     int k_blocks_per_split;
     int n_splits;
-    int prefetch;         // L2 prefetch distance in k-blocks (0 = off)
-    int debug;            // timing experiments only (results are WRONG when non-zero): bit0 = skip the hi/lo split,
-                          // bit1 = issue only the hi*hi product, bit2 = epilogue skips the global stores
-    // ---- TS kernel only (zero-initialised elsewhere) ----
     int k_blocks_a1;      // k-blocks [0, k_blocks_a1) stream from tmap_a, the rest from tmap_a2 (A = [a1 | a2] along K):
-                          // two products accumulate into ONE TMEM accumulator (SAGE: agg W_l^T + x W_r^T)
-    int n_tiles_c1;       // n-tiles [0, n_tiles_c1) are stored through tmap_c, the rest through tmap_c2 (two outputs)
-    const float* bias;    // epilogue: + bias[n] (nullable)
+                          // two products accumulate into ONE accumulator (SAGE: agg W_l^T + x W_r^T)
     int relu;             // epilogue: max(., 0)
-    // ---- grouped (segment_matmul) form of the TS kernel ----
+    // ---- grouped (segment_matmul) form ----
     const int64_t* seg_ptr;   // [n_seg + 1] row offsets of the segments of A / C (device memory: no host read of the sizes)
     int n_seg;                // segment r multiplies with B block r
-    int b_seg_rows;           // rows of the stacked B matrix per segment (K for a [R, K, N] weight read MN-major, N_out K-major)
+    int b_seg_rows;           // rows of the stacked B matrix per segment
 };
 
-// A_MN / B_MN: operand is MN-major (stored row-major as [K, MN]); B_PRE: B arrives pre-split
-// (two tensor maps: hi, lo) so only A is split in shared memory.
-template <int BN, int BK, bool A_MN, bool B_MN, bool B_PRE>
+struct Tile {
+    int64_t m0;           // first output row
+    int n0, seg, rows, split;
+};
+// w -> tile; GROUPED: tiles never straddle a segment (the last tile of a segment is partial)
+template <bool GROUPED>
+__device__ __forceinline__ bool decode_tile(int w, const GemmArgs& args, const int* tile_prefix, Tile& t) {
+    const int tiles_per_split = (GROUPED ? tile_prefix[args.n_seg] : args.n_tiles_m) * args.n_tiles_n;
+    t.split = w / tiles_per_split;
+    const int r0 = w - t.split * tiles_per_split;
+    const int mt = r0 / args.n_tiles_n;                  // n fastest: the column tiles of a row block are adjacent
+    t.n0 = r0 % args.n_tiles_n;
+    if (!GROUPED) {
+        t.m0 = static_cast<int64_t>(mt) * kBM;
+        t.seg = 0;
+        t.rows = static_cast<int>(args.m - t.m0 < kBM ? args.m - t.m0 : kBM);
+        return true;
+    }
+    int r = 0;
+    while (r < args.n_seg && tile_prefix[r + 1] <= mt) ++r;          // few segments: a linear scan of shared memory
+    if (r >= args.n_seg) return false;
+    const int64_t s1 = args.seg_ptr[r + 1];
+    t.m0 = args.seg_ptr[r] + static_cast<int64_t>(mt - tile_prefix[r]) * kBM;
+    t.seg = r;
+    t.rows = static_cast<int>(s1 - t.m0 < kBM ? s1 - t.m0 : kBM);
+    return true;
+}
+
+// A_MN / B_MN: operand is MN-major (stored row-major as [K, MN]); B_PRE: B arrives pre-split (tmap_b_hi,
+// tmap_b_lo), else tmap_b_hi is the raw matrix and the consumers split it.
+template <int BN, bool A_MN, bool B_MN, bool B_PRE, bool GROUPED>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b_hi,
-                   const __grid_constant__ CUtensorMap tmap_b_lo, GemmArgs args) {
-    constexpr int kStages = BK == 32 ? 2 : 4;
-    constexpr int kBK = BK;
-    constexpr uint32_t kSlab = BK * 128;                        // one MN-major slab: BK k-rows x 32 MN elements
-    constexpr uint32_t kABytes = kBM * BK * 4;                  // 128 rows x BK fp32 (either major)
-    constexpr uint32_t kBBytes = BN * BK * 4;
-    constexpr uint32_t kStageBytes = 2 * kABytes + 2 * kBBytes;
-    constexpr uint32_t kTxBytes = kABytes + (B_PRE ? 2 : 1) * kBBytes;
-    constexpr uint32_t kTmemCols = kAccStages * BN;             // 512 for BN = 256
-    constexpr uint32_t kIdesc = instr_desc(kBM, BN, A_MN, B_MN);
+gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
+                   const __grid_constant__ CUtensorMap tmap_b_hi, const __grid_constant__ CUtensorMap tmap_b_lo, GemmArgs args) {
+    constexpr uint32_t kABytes = kBM * kBK * 4;                 // 16 KB
+    constexpr uint32_t kBBytes = BN * kBK * 4;
+    constexpr uint32_t kStageBytes = kABytes + (B_PRE ? 2 : 1) * kBBytes;
+    constexpr uint32_t kTxBytes = kStageBytes;
+    constexpr int kAcc = BN / 2;                                // fp32 accumulators per thread (m64 x BN per warpgroup)
 
     extern __shared__ __align__(1024) unsigned char gemm_smem[];
     const uint32_t smem_base = (s2u(gemm_smem) + 1023u) & ~1023u;
     unsigned char* smem_gen = gemm_smem + (smem_base - s2u(gemm_smem));
-    const uint32_t bars = smem_base + kStages * kStageBytes;
-    // barrier slots (8 B each): full[s], split[s], empty[s], tmem_full[a], tmem_empty[a]
+    const uint32_t b_hi_buf = smem_base + kStages * kStageBytes;  // split B (K-major, 128B swizzle), shared by both warpgroups
+    const uint32_t b_lo_buf = b_hi_buf + kBBytes;
+    const uint32_t bars = b_lo_buf + kBBytes;
     auto bar_full = [&](int s) { return bars + 8u * s; };
-    auto bar_split = [&](int s) { return bars + 8u * (kStages + s); };
-    auto bar_empty = [&](int s) { return bars + 8u * (2 * kStages + s); };
-    auto bar_tfull = [&](int a) { return bars + 8u * (3 * kStages + a); };
-    auto bar_tempty = [&](int a) { return bars + 8u * (3 * kStages + kAccStages + a); };
-    const uint32_t tmem_slot = bars + 8u * (3 * kStages + 2 * kAccStages);
-    volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
+    auto bar_empty = [&](int s) { return bars + 8u * (kStages + s); };
 
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-
+    __shared__ int tile_prefix[GROUPED ? kMaxSegments + 2 : 1];
+    if (GROUPED && threadIdx.x == 32) {                          // tiles of 128 rows per segment, exclusive prefix
+        int acc = 0;
+        for (int r = 0; r < args.n_seg; ++r) {
+            tile_prefix[r] = acc;
+            acc += static_cast<int>((args.seg_ptr[r + 1] - args.seg_ptr[r] + kBM - 1) / kBM);
+        }
+        tile_prefix[args.n_seg] = acc;
+    }
     if (threadIdx.x == 0) {
         for (int s = 0; s < kStages; ++s) {
             bar_init(bar_full(s), 1);
-            bar_init(bar_split(s), 128);
-            bar_init(bar_empty(s), 1);
-        }
-        for (int a = 0; a < kAccStages; ++a) {
-            bar_init(bar_tfull(a), 1);
-            bar_init(bar_tempty(a), 128);
+            bar_init(bar_empty(s), kConsumerThreads / 32);       // one arrive per consumer warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) tmem_alloc(tmem_slot, kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
 
-    const int tiles_per_split = args.n_tiles_m * args.n_tiles_n;
-    const int n_work = tiles_per_split * args.n_splits;
+    const int n_work = (GROUPED ? tile_prefix[args.n_seg] : args.n_tiles_m) * args.n_tiles_n * args.n_splits;
+    const int wg = threadIdx.x >> 7;
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ===================== TMA producer =====================
-        if (lane == 0) {
+        if (threadIdx.x == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-                const int split = w / tiles_per_split;
-                const int t = w - split * tiles_per_split;
-                const int m0 = (t / args.n_tiles_n) * kBM;
-                const int n0 = (t % args.n_tiles_n) * BN;
-                const int kb0 = split * args.k_blocks_per_split;
+                Tile t;
+                decode_tile<GROUPED>(w, args, tile_prefix, t);
+                const int m0 = static_cast<int>(t.m0), n0 = t.n0 * BN;
+                const int b_row0 = GROUPED ? t.seg * args.b_seg_rows : 0;       // this segment's block of the stacked B
+                const int kb0 = t.split * args.k_blocks_per_split;
                 const int kb1 = min(kb0 + args.k_blocks_per_split, args.k_blocks);
                 for (int kb = kb0; kb < kb1; ++kb) {
-                    if (args.prefetch > 0) {
-                        // streaming operands (A always, B when it is not the pre-split weight) `prefetch` k-blocks ahead
-                        int pk = kb + args.prefetch, pm0 = m0;
-                        bool ok = pk < kb1;
-                        if (!ok && args.n_splits == 1 && w + static_cast<int>(gridDim.x) < n_work) {
-                            pk = kb0 + (pk - kb1);                                  // wraps into this CTA's next tile
-                            pm0 = ((w + static_cast<int>(gridDim.x)) / args.n_tiles_n) * kBM;
-                            ok = pk < kb1;
-                        }
-                        if (ok) {
-                            if (A_MN) {
-#pragma unroll
-                                for (int s = 0; s < kBM / 32; ++s) tma_prefetch_2d(&tmap_a, pm0 + 32 * s, pk * kBK);
-                            } else {
-                                tma_prefetch_2d(&tmap_a, pk * kBK, pm0);
-                            }
-                            if (!B_PRE && B_MN) {
-#pragma unroll
-                                for (int s = 0; s < BN / 32; ++s) tma_prefetch_2d(&tmap_b_hi, n0 + 32 * s, pk * kBK);
-                            }
-                        }
-                    }
                     bar_wait(bar_empty(stage), phase ^ 1u);
                     const uint32_t sa = smem_base + stage * kStageBytes;
-                    const uint32_t sb_hi = sa + 2 * kABytes;
-                    const uint32_t sb_lo = sb_hi + kBBytes;
+                    const uint32_t sb = sa + kABytes;
                     bar_expect_tx(bar_full(stage), kTxBytes);
-                    if (A_MN) {
-#pragma unroll
-                        for (int s = 0; s < kBM / 32; ++s) tma_load_2d(sa + s * kSlab, &tmap_a, m0 + 32 * s, kb * kBK, bar_full(stage));
-                    } else {
-                        tma_load_2d(sa, &tmap_a, kb * kBK, m0, bar_full(stage));
-                    }
+                    if (A_MN) tma_load_2d(sa, &tmap_a, m0, kb * kBK, bar_full(stage));
+                    else if (kb < args.k_blocks_a1) tma_load_2d(sa, &tmap_a, kb * kBK, m0, bar_full(stage));
+                    else tma_load_2d(sa, &tmap_a2, (kb - args.k_blocks_a1) * kBK, m0, bar_full(stage));
                     if (B_MN) {
-#pragma unroll
-                        for (int s = 0; s < BN / 32; ++s) {
-                            tma_load_2d(sb_hi + s * kSlab, &tmap_b_hi, n0 + 32 * s, kb * kBK, bar_full(stage));
-                            if (B_PRE) tma_load_2d(sb_lo + s * kSlab, &tmap_b_lo, n0 + 32 * s, kb * kBK, bar_full(stage));
-                        }
+                        tma_load_2d(sb, &tmap_b_hi, n0, b_row0 + kb * kBK, bar_full(stage));
+                        if (B_PRE) tma_load_2d(sb + kBBytes, &tmap_b_lo, n0, b_row0 + kb * kBK, bar_full(stage));
                     } else {
-                        tma_load_2d(sb_hi, &tmap_b_hi, kb * kBK, n0, bar_full(stage));
-                        if (B_PRE) tma_load_2d(sb_lo, &tmap_b_lo, kb * kBK, n0, bar_full(stage));
+                        tma_load_2d(sb, &tmap_b_hi, kb * kBK, b_row0 + n0, bar_full(stage));
+                        if (B_PRE) tma_load_2d(sb + kBBytes, &tmap_b_lo, kb * kBK, b_row0 + n0, bar_full(stage));
                     }
                     if (++stage == kStages) { stage = 0; phase ^= 1u; }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            int stage = 0, acc = 0;
-            uint32_t phase = 0, acc_phase = 0;
-            for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-                const int split = w / tiles_per_split;
-                const int kb0 = split * args.k_blocks_per_split;
-                const int kb1 = min(kb0 + args.k_blocks_per_split, args.k_blocks);
-                bar_wait(bar_tempty(acc), acc_phase ^ 1u);
-                tc_fence_after();
-                const uint32_t d = tmem_base + static_cast<uint32_t>(acc * BN);
-                uint32_t accumulate = 0;
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    bar_wait(bar_full(stage), phase);      // TMA bytes (incl. the pre-split B tiles) have landed
-                    bar_wait(bar_split(stage), phase);     // hi/lo tiles written and fenced by the splitter
-                    tc_fence_after();
-                    const uint32_t sa_hi = smem_base + stage * kStageBytes;
-                    const uint32_t sa_lo = sa_hi + kABytes;
-                    const uint32_t sb_hi = sa_hi + 2 * kABytes;
-                    const uint32_t sb_lo = sb_hi + kBBytes;
+        return;
+    }
+
+    // ===================== consumers: warpgroups 1 and 2 =====================
+    const int ct = threadIdx.x - 128;                           // 0..255 across both consumer warpgroups
+    const int lane = threadIdx.x & 31;
+    const int row_base = (wg - 1) * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // fragment rows row_base, +8
+    const int kq = lane & 3;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[kAcc];
+    for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
+        Tile t;
+        decode_tile<GROUPED>(w, args, tile_prefix, t);
+        const int kb0 = t.split * args.k_blocks_per_split;
+        const int kb1 = min(kb0 + args.k_blocks_per_split, args.k_blocks);
 #pragma unroll
-                    for (int j = 0; j < kBK / 8; ++j) {
-                        // K-major: 8 tf32 = 32 B further along the 128-byte swizzle row;
-                        // MN-major: the next group of 8 k-rows = 1024 B further.
-                        const uint32_t ao = A_MN ? j * 1024u : j * 32u;
-                        const uint32_t bo = B_MN ? j * 1024u : j * 32u;
-                        const uint64_t a_hi = smem_desc<A_MN, BK>(sa_hi + ao, kSlab);
-                        const uint64_t a_lo = smem_desc<A_MN, BK>(sa_lo + ao, kSlab);
-                        const uint64_t b_hi = smem_desc<B_MN, BK>(sb_hi + bo, kSlab);
-                        const uint64_t b_lo = smem_desc<B_MN, BK>(sb_lo + bo, kSlab);
-                        if (!(args.debug & 2)) {
-                            umma_tf32(d, a_lo, b_hi, kIdesc, accumulate);     // small terms first
-                            umma_tf32(d, a_hi, b_lo, kIdesc, 1u);
-                            umma_tf32(d, a_hi, b_hi, kIdesc, 1u);
+        for (int i = 0; i < kAcc; ++i) acc[i] = 0.0f;
+        for (int kb = kb0; kb < kb1; ++kb) {
+            bar_wait(bar_full(stage), phase);
+            const unsigned char* sa = smem_gen + stage * kStageBytes;
+            const unsigned char* sb = sa + kABytes;
+            // (1) B tile -> (hi, lo), K-major 128B swizzle.  Both warpgroups finished their previous wgmmas
+            // (wait_group 0) before this barrier, so the split buffers are free.
+            consumer_sync();
+            unsigned char* bh = smem_gen + (b_hi_buf - smem_base);
+            unsigned char* bl = smem_gen + (b_lo_buf - smem_base);
+            if (!B_MN) {
+                // raw TMA tile already has the target layout: element-wise
+#pragma unroll
+                for (uint32_t off = ct * 16u; off < kBBytes; off += kConsumerThreads * 16u) {
+                    const float4 v = *reinterpret_cast<const float4*>(sb + off);
+                    float4 h, l;
+                    if (B_PRE) {
+                        h = v;
+                        l = *reinterpret_cast<const float4*>(sb + kBBytes + off);
+                    } else {
+                        h = make_float4(rn_tf32(v.x), rn_tf32(v.y), rn_tf32(v.z), rn_tf32(v.w));
+                        l = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
+                    }
+                    *reinterpret_cast<float4*>(bh + off) = h;
+                    *reinterpret_cast<float4*>(bl + off) = l;
+                }
+            } else {
+                // raw tile is [32 k][BN n] (unswizzled): gather 4 consecutive k of one n, store one 16-byte chunk
+                const float* rb = reinterpret_cast<const float*>(sb);
+#pragma unroll
+                for (int idx = ct; idx < BN * 8; idx += kConsumerThreads) {
+                    const int n = idx % BN, kc = idx / BN;
+                    float v[4], h[4], l[4];
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) v[i] = rb[(4 * kc + i) * BN + n];
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        if (B_PRE) {
+                            h[i] = v[i];
+                            l[i] = rb[BN * kBK + (4 * kc + i) * BN + n];
                         } else {
-                            umma_tf32(d, a_hi, b_hi, kIdesc, accumulate);
+                            h[i] = rn_tf32(v[i]);
+                            l[i] = v[i] - h[i];
                         }
-                        accumulate = 1u;
                     }
-                    umma_commit(bar_empty(stage));                        // frees the smem stage when the MMAs retire
-                    if (++stage == kStages) { stage = 0; phase ^= 1u; }
+                    const uint32_t off = sw128_offset(n, 4 * kc);
+                    *reinterpret_cast<float4*>(bh + off) = make_float4(h[0], h[1], h[2], h[3]);
+                    *reinterpret_cast<float4*>(bl + off) = make_float4(l[0], l[1], l[2], l[3]);
                 }
-                umma_commit(bar_tfull(acc));                              // accumulator complete
-                if (++acc == kAccStages) { acc = 0; acc_phase ^= 1u; }
             }
-        }
-    } else if (warp >= 4 && warp < 8) {
-        // ===================== splitter (128 threads) =====================
-        const int tid = threadIdx.x - 128;
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-            const int split = w / tiles_per_split;
-            const int kb0 = split * args.k_blocks_per_split;
-            const int kb1 = min(kb0 + args.k_blocks_per_split, args.k_blocks);
-            for (int kb = kb0; kb < kb1; ++kb) {
-                bar_wait(bar_full(stage), phase);
-                unsigned char* sa = smem_gen + stage * kStageBytes;
-                auto split_buf = [&](unsigned char* hi, unsigned char* lo, int bytes) {
-                    for (int off = tid * 16; off < bytes; off += 128 * 16) {
-                        float4 v = *reinterpret_cast<float4*>(hi + off);
-                        float4 h = make_float4(rn_tf32(v.x), rn_tf32(v.y), rn_tf32(v.z), rn_tf32(v.w));
-                        float4 l = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
-                        *reinterpret_cast<float4*>(hi + off) = h;
-                        *reinterpret_cast<float4*>(lo + off) = l;
-                    }
-                };
-                if (!(args.debug & 1)) {
-                    split_buf(sa, sa + kABytes, kABytes);
-                    if (!B_PRE) split_buf(sa + 2 * kABytes, sa + 2 * kABytes + kBBytes, kBBytes);
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> async (MMA) reads
-                bar_arrive(bar_split(stage));
-                if (++stage == kStages) { stage = 0; phase ^= 1u; }
-            }
-        }
-    } else if (warp >= 8) {
-        // ===================== epilogue (128 threads, TMEM lane quadrant = warp % 4) =====================
-        const int q = warp & 3;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-            const int split = w / tiles_per_split;
-            const int t = w - split * tiles_per_split;
-            const int64_t m0 = static_cast<int64_t>(t / args.n_tiles_n) * kBM;
-            const int n0 = (t % args.n_tiles_n) * BN;
-            bar_wait(bar_tfull(acc), acc_phase);
-            tc_fence_after();
-            const int64_t row = m0 + q * 32 + lane;
-            float* crow = args.c + (static_cast<int64_t>(split) * args.m + row) * args.ldc + n0;
-#pragma unroll 1
-            for (int c0 = 0; c0 < BN; c0 += 32) {
-                uint32_t r[32];
-                tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * BN + c0), r);
-                if (row < args.m && !(args.debug & 4)) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> wgmma (async proxy) reads
+            // (2) A fragments of this warpgroup's 64 rows, split in registers
+            uint32_t a_hi[kBK / 8][4], a_lo[kBK / 8][4];
 #pragma unroll
-                    for (int i = 0; i < 32; i += 8) stg_v8(crow + c0 + i, r + i);   // 256-bit stores: one full 32 B sector each
+            for (int j = 0; j < kBK / 8; ++j) {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int r = row_base + (i & 1) * 8, k = j * 8 + kq + (i >> 1) * 4;
+                    const float v = A_MN ? *reinterpret_cast<const float*>(sa + k * (kBM * 4) + r * 4)
+                                         : *reinterpret_cast<const float*>(sa + sw128_offset(r, k));
+                    const float h = rn_tf32(v);
+                    a_hi[j][i] = __float_as_uint(h);
+                    a_lo[j][i] = __float_as_uint(v - h);
                 }
             }
-            tc_fence_before();
-            bar_arrive(bar_tempty(acc));
-            if (++acc == kAccStages) { acc = 0; acc_phase ^= 1u; }
+            consumer_sync();                                       // split B visible to both warpgroups
+            __syncwarp();
+            if (lane == 0) bar_arrive(bar_empty(stage));           // raw A and B of this stage are consumed
+            // (3) 4 k-steps x 3 products, small terms first
+            fence_regs(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int j = 0; j < kBK / 8; ++j) {
+                const uint64_t dh = smem_desc_sw128(b_hi_buf + j * 32u);
+                const uint64_t dl = smem_desc_sw128(b_lo_buf + j * 32u);
+                wgmma_tf32<BN>(acc, a_lo[j], dh, (kb > kb0 || j > 0) ? 1u : 0u);
+                wgmma_tf32<BN>(acc, a_hi[j], dl, 1u);
+                wgmma_tf32<BN>(acc, a_hi[j], dh, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait_all();
+            fence_regs(acc);
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+        }
+        // ===================== epilogue: fragments -> global, rows masked =====================
+        const int nt = t.n0;
+        const bool second = nt >= args.n_tiles_c1;
+        float* out = second ? args.c2 : args.c;
+        const int64_t ldc = second ? args.ldc2 : args.ldc;
+        const int col0 = (second ? nt - args.n_tiles_c1 : nt) * BN;
+        const int bias0 = nt * BN;
+        float* base = out + static_cast<int64_t>(t.split) * args.m * ldc;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = row_base + h * 8;
+            if (r >= t.rows) continue;
+            float* dst = base + (t.m0 + r) * ldc + col0;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int c = j * 8 + 2 * kq;
+                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                if (args.bias) {
+                    v0 += __ldg(args.bias + bias0 + c);
+                    v1 += __ldg(args.bias + bias0 + c + 1);
+                }
+                if (args.relu) {
+                    v0 = fmaxf(v0, 0.0f);
+                    v1 = fmaxf(v1, 0.0f);
+                }
+                *reinterpret_cast<float2*>(dst + c) = make_float2(v0, v1);
+            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // w -> (rn_tf32(w), w - rn_tf32(w)) for the (small) weight matrix
@@ -439,15 +413,13 @@ static EncodeTiledFn encode_fn() {
     }
     return fn;
 }
-// 2-D fp32 row-major [rows, cols] tensor, zero fill.
-//   K-major operand  (mn = false): box = [box_rows, bk cols], 128B (bk = 32) or 64B (bk = 16) swizzle;
-//   MN-major operand (mn = true) : box = [bk k-rows, 32 MN cols], 128B swizzle with a 32-byte atom.
-static int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t cols, int64_t ld, bool mn, int bk,
-                    int box_rows) {
-    const CUtensorMapSwizzle swz = mn ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B
-                                      : (bk == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
-    const int box_cols = mn ? 32 : bk;
-    if (mn) box_rows = bk;
+// 2-D fp32 row-major [rows, cols] tensor, zero fill out of bounds.
+//   K-major operand  (mn = false): box = [box_mn rows, 32 cols], 128B swizzle (the wgmma K-major layout);
+//   MN-major operand (mn = true) : box = [32 k-rows, box_mn cols], unswizzled (transposed while it is split).
+static int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t cols, int64_t ld, bool mn, int box_mn) {
+    const CUtensorMapSwizzle swz = mn ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B;
+    const int box_cols = mn ? box_mn : kBK;
+    const int box_rows = mn ? kBK : box_mn;
     EncodeTiledFn fn = encode_fn();
     // cuTensorMapEncodeTiled is a DRIVER call: it needs a current context.  On a fresh thread (the
     // autograd engine's backward thread) no runtime call may have bound the primary context yet.
@@ -464,117 +436,76 @@ static int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t c
                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
-        set_error("cuTensorMapEncodeTiled failed (%d) rows=%lld cols=%lld ld=%lld box_rows=%d", static_cast<int>(r),
-                  static_cast<long long>(rows), static_cast<long long>(cols), static_cast<long long>(ld), box_rows);
+        set_error("cuTensorMapEncodeTiled failed (%d) rows=%lld cols=%lld ld=%lld box_mn=%d", static_cast<int>(r),
+                  static_cast<long long>(rows), static_cast<long long>(cols), static_cast<long long>(ld), box_mn);
         return B200MP_ERR_CUDA;
     }
     return B200MP_OK;
 }
 
-template <int BN, int BK, bool A_MN, bool B_MN, bool B_PRE>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tbh, const CUtensorMap& tbl, const GemmArgs& args,
-                       cudaStream_t stream) {
-    constexpr size_t smem = (BK == 32 ? 2 : 4) * (2 * kBM * BK * 4 + 2 * BN * BK * 4) + 256 + 1024;
-    auto kfn = gemm_tf32x3_kernel<BN, BK, A_MN, B_MN, B_PRE>;
+template <int BN, bool A_MN, bool B_MN, bool B_PRE, bool GROUPED = false>
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& ta2, const CUtensorMap& tbh, const CUtensorMap& tbl,
+                       const GemmArgs& args, int n_work, cudaStream_t stream) {
+    constexpr size_t smem = kStages * (kBM * kBK * 4 + (B_PRE ? 2 : 1) * BN * kBK * 4) + 2 * BN * kBK * 4 + 8 * 2 * kStages + 1024;
+    static_assert(smem <= 227 * 1024, "one CTA per SM must fit the 227 KB opt-in shared memory of sm_90");
+    auto kfn = gemm_tf32x3_kernel<BN, A_MN, B_MN, B_PRE, GROUPED>;
     B200MP_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    const int n_work = args.n_tiles_m * args.n_tiles_n * args.n_splits;
     const int grid = n_work < num_sms() ? n_work : num_sms();
-    kfn<<<grid, kGemmThreads, smem, stream>>>(ta, tbh, tbl, args);
+    kfn<<<grid, kGemmThreads, smem, stream>>>(ta, ta2, tbh, tbl, args);
     B200MP_LAUNCH_CHECK();
     return B200MP_OK;
 }
+// BN = 64 only for a 64-wide output, else 128 (every supported width is then a multiple of it)
+template <bool A_MN, bool B_MN, bool B_PRE>
+static int launch_bn(int bn, const CUtensorMap& ta, const CUtensorMap& ta2, const CUtensorMap& tbh, const CUtensorMap& tbl,
+                     const GemmArgs& args, cudaStream_t s) {
+    const int n_work = args.n_tiles_m * args.n_tiles_n * args.n_splits;
+    return bn == 64 ? launch_gemm<64, A_MN, B_MN, B_PRE>(ta, ta2, tbh, tbl, args, n_work, s)
+                    : launch_gemm<128, A_MN, B_MN, B_PRE>(ta, ta2, tbh, tbl, args, n_work, s);
+}
 
 static bool ok16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
-}  // namespace b200mp
-
-#include "gemm_tf32x3_ts.cuh"
-
-using namespace b200mp;
-
-namespace b200mp {
-int get_option_gemm_bk();   // 16 or 32 (b200mp_set_option("gemm_bk", ...)); default = measured best
-int get_option_gemm_mode(); // 0 = SS (A and B in shared memory), 1 = TS (A operand in tensor memory)
-int get_option_gemm_debug();
-int get_option_gemm_prefetch(); // L2 prefetch distance in k-blocks for the streaming operands (0 = off)
-
 static bool width_ok(int64_t w) { return w == 64 || w == 128 || (w > 0 && w % 256 == 0); }
+static int tile_n(int64_t w) { return w == 64 ? 64 : 128; }
 
-// TS path (A in TMEM): [c1 | c2][M, n1 + n2] = [a1 | a2][M, k1 + k2] . B (+ bias, relu), K-major or MN-major B;
-// b_lo == nullptr: b_hi is the unsplit matrix and the kernel splits the B tiles itself
-static int run_ts2(const float* a1, int64_t k1, const float* a2, int64_t k2, const float* b_hi, const float* b_lo, float* c1,
-                   int64_t n1, float* c2, int64_t n2, const float* bias, int relu, int64_t m, bool b_mn, cudaStream_t s) {
+// [c1 | c2][M, n1 + n2] = [a1 | a2][M, k1 + k2] . B (+ bias, relu), B K-major ([n_out, k_red]) or MN-major
+// ([k_red, n_out]); b_lo == nullptr: b_hi is the unsplit matrix and the kernel splits the B tiles itself
+static int run_pair(const float* a1, int64_t k1, const float* a2, int64_t k2, const float* b_hi, const float* b_lo, float* c1,
+                    int64_t n1, float* c2, int64_t n2, const float* bias, int relu, int64_t m, bool b_mn, cudaStream_t s) {
     const int64_t k_red = k1 + k2, n_out = n1 + n2;
     const int64_t b_rows = b_mn ? k_red : n_out, b_cols = b_mn ? n_out : k_red;
-    CUtensorMap ta, ta2, tbh, tbl, tc, tc2;
+    const int bn = (n1 == 64 && n2 == 0) ? 64 : 128;
+    CUtensorMap ta, ta2, tbh, tbl;
     int rc;
-    if ((rc = make_map(&tc, c1, m, n1, n1, false, 32, 32))) return rc;           // output boxes [32 rows x 32 cols]
-    if ((rc = make_map(&tc2, c2 ? c2 : c1, m, c2 ? n2 : n1, c2 ? n2 : n1, false, 32, 32))) return rc;
-    if ((rc = make_map(&ta, a1, m, k1, k1, false, 32, kBM))) return rc;
-    if ((rc = make_map(&ta2, a2 ? a2 : a1, m, a2 ? k2 : k1, a2 ? k2 : k1, false, 32, kBM))) return rc;
-    if ((rc = make_map(&tbh, b_hi, b_rows, b_cols, b_cols, b_mn, 32, kTsBN))) return rc;
-    if ((rc = make_map(&tbl, b_lo ? b_lo : b_hi, b_rows, b_cols, b_cols, b_mn, 32, kTsBN))) return rc;
-    const int kb = static_cast<int>(k_red / 32);
-    GemmArgs args{c1, m, n_out, static_cast<int>(ceil_div(m, kBM)), static_cast<int>(n_out / kTsBN), kb, kb, 1,
-                  get_option_gemm_prefetch(), get_option_gemm_debug(), static_cast<int>(k1 / 32), static_cast<int>(n1 / kTsBN), bias, relu};
-    if (!b_lo) return b_mn ? launch_gemm_ts<true, true>(ta, ta2, tbh, tbl, tc, tc2, args, s) : launch_gemm_ts<false, true>(ta, ta2, tbh, tbl, tc, tc2, args, s);
-    return b_mn ? launch_gemm_ts<true, false>(ta, ta2, tbh, tbl, tc, tc2, args, s) : launch_gemm_ts<false, false>(ta, ta2, tbh, tbl, tc, tc2, args, s);
-}
-static int run_ts(const float* a, const float* b_hi, const float* b_lo, float* c, int64_t m, int64_t n_out, int64_t k_red,
-                  bool b_mn, int64_t b_rows, int64_t b_cols, cudaStream_t s) {
-    (void)b_rows; (void)b_cols;
-    return run_ts2(a, k_red, nullptr, 0, b_hi, b_lo, c, n_out, nullptr, 0, nullptr, 0, m, b_mn, s);
+    if ((rc = make_map(&ta, a1, m, k1, k1, false, kBM))) return rc;
+    if ((rc = make_map(&ta2, a2 ? a2 : a1, m, a2 ? k2 : k1, a2 ? k2 : k1, false, kBM))) return rc;
+    if ((rc = make_map(&tbh, b_hi, b_rows, b_cols, b_cols, b_mn, bn))) return rc;
+    if ((rc = make_map(&tbl, b_lo ? b_lo : b_hi, b_rows, b_cols, b_cols, b_mn, bn))) return rc;
+    const int kb = static_cast<int>(k_red / kBK);
+    GemmArgs args{};
+    args.c = c1;
+    args.c2 = c2;
+    args.bias = bias;
+    args.m = m;
+    args.ldc = n1;
+    args.ldc2 = n2;
+    args.n_tiles_m = static_cast<int>(ceil_div(m, kBM));
+    args.n_tiles_n = static_cast<int>(n_out / bn);
+    args.n_tiles_c1 = static_cast<int>(n1 / bn);
+    args.k_blocks = args.k_blocks_per_split = kb;
+    args.n_splits = 1;
+    args.k_blocks_a1 = static_cast<int>(k1 / kBK);
+    args.relu = relu;
+    if (b_lo) return b_mn ? launch_bn<false, true, true>(bn, ta, ta2, tbh, tbl, args, s) : launch_bn<false, false, true>(bn, ta, ta2, tbh, tbl, args, s);
+    return b_mn ? launch_bn<false, true, false>(bn, ta, ta2, tbh, tbl, args, s) : launch_bn<false, false, false>(bn, ta, ta2, tbh, tbl, args, s);
 }
 
-// y[M,N] = x[M,K] . w[N,K]^T
-template <int BK>
-static int run_forward(const float* x, const float* w_hi, const float* w_lo, float* y, int64_t m, int64_t n, int64_t k,
-                       cudaStream_t s) {
-    if ((get_option_gemm_mode() == 1 || !w_lo) && n % kTsBN == 0) return run_ts(x, w_hi, w_lo, y, m, n, k, false, n, k, s);
-    if (!w_lo) {
-        set_error("linear_tf32x3: an unsplit weight (w_lo == NULL) needs an output width that is a multiple of %d", kTsBN);
-        return B200MP_ERR_UNSUPPORTED;
-    }
-    const int bn = n >= 256 ? 256 : static_cast<int>(n);
-    CUtensorMap ta, tbh, tbl;
-    int rc;
-    if ((rc = make_map(&ta, x, m, k, k, false, BK, kBM))) return rc;
-    if ((rc = make_map(&tbh, w_hi, n, k, k, false, BK, bn))) return rc;
-    if ((rc = make_map(&tbl, w_lo, n, k, k, false, BK, bn))) return rc;
-    const int kb = static_cast<int>(k / BK);
-    GemmArgs a{y, m, n, static_cast<int>(ceil_div(m, kBM)), static_cast<int>(n / bn), kb, kb, 1, get_option_gemm_prefetch(), get_option_gemm_debug()};
-    if (bn == 256) return launch_gemm<256, BK, false, false, true>(ta, tbh, tbl, a, s);
-    if (bn == 128) return launch_gemm<128, BK, false, false, true>(ta, tbh, tbl, a, s);
-    return launch_gemm<64, BK, false, false, true>(ta, tbh, tbl, a, s);
-}
-// gx[M,K] = g[M,N] . w[N,K]   (B = w read MN-major exactly as stored: [K' = n rows][N' = k cols])
-template <int BK>
-static int run_grad_input(const float* g, const float* w_hi, const float* w_lo, float* gx, int64_t m, int64_t n, int64_t k,
-                          cudaStream_t s) {
-    if ((get_option_gemm_mode() == 1 || !w_lo) && k % kTsBN == 0) return run_ts(g, w_hi, w_lo, gx, m, k, n, true, n, k, s);
-    if (!w_lo) {
-        set_error("linear_grad_input_tf32x3: an unsplit weight (w_lo == NULL) needs an input width that is a multiple of %d", kTsBN);
-        return B200MP_ERR_UNSUPPORTED;
-    }
-    const int bn = k >= 256 ? 256 : static_cast<int>(k);
-    CUtensorMap ta, tbh, tbl;
-    int rc;
-    if ((rc = make_map(&ta, g, m, n, n, false, BK, kBM))) return rc;
-    if ((rc = make_map(&tbh, w_hi, n, k, k, true, BK, 0))) return rc;
-    if ((rc = make_map(&tbl, w_lo, n, k, k, true, BK, 0))) return rc;
-    const int kb = static_cast<int>(n / BK);
-    GemmArgs a{gx, m, k, static_cast<int>(ceil_div(m, kBM)), static_cast<int>(k / bn), kb, kb, 1, get_option_gemm_prefetch(), get_option_gemm_debug()};
-    if (bn == 256) return launch_gemm<256, BK, false, true, true>(ta, tbh, tbl, a, s);
-    if (bn == 128) return launch_gemm<128, BK, false, true, true>(ta, tbh, tbl, a, s);
-    return launch_gemm<64, BK, false, true, true>(ta, tbh, tbl, a, s);
-}
 // gw[N,K] = g[M,N]^T . x[M,K]: both operands MN-major as stored, split-K over the M rows
-template <int BK>
 static int run_grad_weight(const float* g, const float* x, float* gw, int64_t m, int64_t n, int64_t k, void* workspace,
                            int64_t workspace_bytes, cudaStream_t s) {
-    const int bn = k >= 256 ? 256 : static_cast<int>(k);
+    const int bn = tile_n(k);
     const int tiles = static_cast<int>((n / kBM) * (k / bn));
-    const int64_t kblocks = ceil_div(m, BK);
+    const int64_t kblocks = ceil_div(m, kBK);
     if (kblocks > 0x7fffffffLL) return B200MP_ERR_UNSUPPORTED;
     int splits = num_sms() / tiles;
     if (splits < 1) splits = 1;
@@ -587,14 +518,19 @@ static int run_grad_weight(const float* g, const float* x, float* gw, int64_t m,
     }
     CUtensorMap ta, tb;
     int rc;
-    if ((rc = make_map(&ta, g, m, n, n, true, BK, 0))) return rc;   // A[m' = n-index, k' = row]: stored [K' rows][M' cols]
-    if ((rc = make_map(&tb, x, m, k, k, true, BK, 0))) return rc;
-    GemmArgs a{static_cast<float*>(workspace), n, k, static_cast<int>(n / kBM), static_cast<int>(k / bn),
-               static_cast<int>(kblocks), kbps, splits, get_option_gemm_prefetch(), get_option_gemm_debug()};
-    if (bn == 256) rc = launch_gemm<256, BK, true, true, false>(ta, tb, tb, a, s);
-    else if (bn == 128) rc = launch_gemm<128, BK, true, true, false>(ta, tb, tb, a, s);
-    else rc = launch_gemm<64, BK, true, true, false>(ta, tb, tb, a, s);
-    if (rc) return rc;
+    if ((rc = make_map(&ta, g, m, n, n, true, kBM))) return rc;    // A[m' = n-index, k' = row]: stored [K' rows][M' cols]
+    if ((rc = make_map(&tb, x, m, k, k, true, bn))) return rc;
+    GemmArgs args{};
+    args.c = static_cast<float*>(workspace);
+    args.m = n;
+    args.ldc = k;
+    args.n_tiles_m = static_cast<int>(n / kBM);
+    args.n_tiles_n = args.n_tiles_c1 = static_cast<int>(k / bn);
+    args.k_blocks = static_cast<int>(kblocks);
+    args.k_blocks_per_split = kbps;
+    args.n_splits = splits;
+    args.k_blocks_a1 = static_cast<int>(kblocks);
+    if ((rc = launch_bn<true, true, false>(bn, ta, ta, tb, tb, args, s))) return rc;
     const int64_t total = n * k;
     splitk_reduce_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, s>>>(static_cast<const float*>(workspace), gw,
                                                                                       total, splits);
@@ -602,6 +538,8 @@ static int run_grad_weight(const float* g, const float* x, float* gw, int64_t m,
     return B200MP_OK;
 }
 }  // namespace b200mp
+
+using namespace b200mp;
 
 extern "C" int b200mp_split_tf32(const float* w, float* w_hi, float* w_lo, int64_t n, void* stream) {
     B200MP_CHECK_ARG(n >= 0);
@@ -612,6 +550,7 @@ extern "C" int b200mp_split_tf32(const float* w, float* w_hi, float* w_lo, int64
     return B200MP_OK;
 }
 
+// y[M,N] = x[M,K] . w[N,K]^T
 extern "C" int b200mp_linear_tf32x3(const float* x, const float* w_hi, const float* w_lo, float* y, int64_t m, int64_t n,
                                     int64_t k, void* stream) {
     B200MP_CHECK_ARG(m >= 0 && n > 0 && k > 0);
@@ -621,10 +560,10 @@ extern "C" int b200mp_linear_tf32x3(const float* x, const float* w_hi, const flo
         set_error("linear_tf32x3: unsupported shape m=%lld n=%lld k=%lld", (long long)m, (long long)n, (long long)k);
         return B200MP_ERR_UNSUPPORTED;
     }
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    return get_option_gemm_bk() == 32 ? run_forward<32>(x, w_hi, w_lo, y, m, n, k, s) : run_forward<16>(x, w_hi, w_lo, y, m, n, k, s);
+    return run_pair(x, k, nullptr, 0, w_hi, w_lo, y, n, nullptr, 0, nullptr, 0, m, false, static_cast<cudaStream_t>(stream));
 }
 
+// gx[M,K] = g[M,N] . w[N,K]   (B = w read MN-major exactly as stored: [K' = n rows][N' = k cols])
 extern "C" int b200mp_linear_grad_input_tf32x3(const float* g, const float* w_hi, const float* w_lo, float* gx, int64_t m,
                                                int64_t n, int64_t k, void* stream) {
     B200MP_CHECK_ARG(m >= 0 && n > 0 && k > 0);
@@ -634,9 +573,7 @@ extern "C" int b200mp_linear_grad_input_tf32x3(const float* g, const float* w_hi
         set_error("linear_grad_input_tf32x3: unsupported shape m=%lld n=%lld k=%lld", (long long)m, (long long)n, (long long)k);
         return B200MP_ERR_UNSUPPORTED;
     }
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    return get_option_gemm_bk() == 32 ? run_grad_input<32>(g, w_hi, w_lo, gx, m, n, k, s)
-                                      : run_grad_input<16>(g, w_hi, w_lo, gx, m, n, k, s);
+    return run_pair(g, n, nullptr, 0, w_hi, w_lo, gx, k, nullptr, 0, nullptr, 0, m, true, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int64_t b200mp_linear_grad_weight_workspace_bytes(int64_t m, int64_t n, int64_t k) {
@@ -657,8 +594,7 @@ extern "C" int b200mp_linear_grad_weight_tf32x3(const float* g, const float* x, 
         set_error("linear_grad_weight_tf32x3: unsupported shape m=%lld n=%lld k=%lld", (long long)m, (long long)n, (long long)k);
         return B200MP_ERR_UNSUPPORTED;
     }
-    return get_option_gemm_bk() == 32 ? run_grad_weight<32>(g, x, gw, m, n, k, workspace, workspace_bytes, s)
-                                      : run_grad_weight<16>(g, x, gw, m, n, k, workspace, workspace_bytes, s);
+    return run_grad_weight(g, x, gw, m, n, k, workspace, workspace_bytes, s);
 }
 
 extern "C" int b200mp_gemm_pair_tf32x3(const float* a1, int64_t k1, const float* a2, int64_t k2, const float* b_hi,
@@ -668,12 +604,12 @@ extern "C" int b200mp_gemm_pair_tf32x3(const float* a1, int64_t k1, const float*
     if (m == 0) return B200MP_OK;
     B200MP_CHECK_ARG(a1 && b_hi && c1 && ok16(a1) && ok16(a2) && ok16(b_hi) && ok16(b_lo) && ok16(c1) && ok16(c2));
     B200MP_CHECK_ARG((k2 == 0) == (a2 == nullptr) && (n2 == 0) == (c2 == nullptr));
-    if (k1 % 32 != 0 || k2 % 32 != 0 || n1 % kTsBN != 0 || n2 % kTsBN != 0 || m > 0x7fffffffLL) {
+    if (k1 % 32 != 0 || k2 % 32 != 0 || n1 % 128 != 0 || n2 % 128 != 0 || m > 0x7fffffffLL) {
         set_error("gemm_pair_tf32x3: unsupported shape m=%lld k=%lld+%lld n=%lld+%lld (k %% 32, n %% 128)", (long long)m,
                   (long long)k1, (long long)k2, (long long)n1, (long long)n2);
         return B200MP_ERR_UNSUPPORTED;
     }
-    return run_ts2(a1, k1, a2, k2, b_hi, b_lo, c1, n1, c2, n2, bias, relu, m, b_layout == 1, static_cast<cudaStream_t>(stream));
+    return run_pair(a1, k1, a2, k2, b_hi, b_lo, c1, n1, c2, n2, bias, relu, m, b_layout == 1, static_cast<cudaStream_t>(stream));
 }
 
 // out[ptr[r] : ptr[r+1]] = a[ptr[r] : ptr[r+1]] . B_r for every segment r in ONE persistent launch: work items are
@@ -684,25 +620,32 @@ extern "C" int b200mp_segment_matmul_tf32x3(const float* a, const int64_t* ptr, 
     B200MP_CHECK_ARG(m >= 0 && k > 0 && n > 0 && n_seg > 0 && (b_layout == 0 || b_layout == 1));
     if (m == 0) return B200MP_OK;
     B200MP_CHECK_ARG(a && ptr && b_hi && b_lo && c && ok16(a) && ok16(b_hi) && ok16(b_lo) && ok16(c));
-    if (k % 32 != 0 || n % kTsBN != 0 || n_seg > kMaxSegments || m > 0x7fffffffLL) {
+    if (k % 32 != 0 || n % 128 != 0 || n_seg > kMaxSegments || m > 0x7fffffffLL) {
         set_error("segment_matmul_tf32x3: unsupported shape m=%lld k=%lld n=%lld segments=%lld (k %% 32, n %% 128, <= 120 segments)",
                   (long long)m, (long long)k, (long long)n, (long long)n_seg);
         return B200MP_ERR_UNSUPPORTED;
     }
     const bool b_mn = b_layout == 1;                       // 1: B_r = w[r] [K, N] row-major (out = a w[r]); 0: B_r = w[r] [N, K] (out = a w[r]^T)
     const int64_t b_rows = n_seg * (b_mn ? k : n), b_cols = b_mn ? n : k;
-    CUtensorMap ta, tbh, tbl, tc;
+    CUtensorMap ta, tbh, tbl;
     int rc;
-    if ((rc = make_map(&tc, c, m, n, n, false, 32, 32))) return rc;
-    if ((rc = make_map(&ta, a, m, k, k, false, 32, kBM))) return rc;
-    if ((rc = make_map(&tbh, b_hi, b_rows, b_cols, b_cols, b_mn, 32, kTsBN))) return rc;
-    if ((rc = make_map(&tbl, b_lo, b_rows, b_cols, b_cols, b_mn, 32, kTsBN))) return rc;
-    const int kb = static_cast<int>(k / 32);
+    if ((rc = make_map(&ta, a, m, k, k, false, kBM))) return rc;
+    if ((rc = make_map(&tbh, b_hi, b_rows, b_cols, b_cols, b_mn, 128))) return rc;
+    if ((rc = make_map(&tbl, b_lo, b_rows, b_cols, b_cols, b_mn, 128))) return rc;
+    const int kb = static_cast<int>(k / kBK);
+    GemmArgs args{};
+    args.c = c;
+    args.m = m;
+    args.ldc = n;
+    args.n_tiles_n = args.n_tiles_c1 = static_cast<int>(n / 128);
+    args.k_blocks = args.k_blocks_per_split = args.k_blocks_a1 = kb;
+    args.n_splits = 1;
+    args.seg_ptr = ptr;
+    args.n_seg = static_cast<int>(n_seg);
+    args.b_seg_rows = static_cast<int>(b_mn ? k : n);
     // upper bound of the work list: every segment adds at most one partial tile
-    const int64_t max_tiles = ceil_div(m, kBM) + n_seg;
-    GemmArgs args{c, m, n, static_cast<int>(max_tiles), static_cast<int>(n / kTsBN), kb, kb, 1, 0, get_option_gemm_debug(),
-                  kb, static_cast<int>(n / kTsBN), nullptr, 0, ptr, static_cast<int>(n_seg), static_cast<int>(b_mn ? k : n)};
+    const int n_work = static_cast<int>((ceil_div(m, kBM) + n_seg) * args.n_tiles_n);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    return b_mn ? launch_gemm_ts<true, false, true>(ta, ta, tbh, tbl, tc, tc, args, s)
-                : launch_gemm_ts<false, false, true>(ta, ta, tbh, tbl, tc, tc, args, s);
+    return b_mn ? launch_gemm<128, false, true, true, true>(ta, ta, tbh, tbl, args, n_work, s)
+                : launch_gemm<128, false, false, true, true>(ta, ta, tbh, tbl, args, n_work, s);
 }

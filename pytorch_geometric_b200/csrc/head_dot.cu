@@ -147,7 +147,7 @@ extern "C" int64_t b200mp_head_dot_parts(int64_t n_rows, int64_t heads, int64_t 
     const int64_t es = val_dtype == B200MP_BF16 ? 2 : 4;
     const int64_t n_vec = heads * chan * es / 16, rps = kHdT / n_vec;
     const int64_t want = ceil_div(n_rows, rps);
-    int sms = 148;
+    int sms = kSMs;
     b200mp_device_info(&sms, nullptr, nullptr, nullptr);
     const int64_t cap = static_cast<int64_t>(sms) * 8;
     return want < cap ? want : cap;

@@ -133,7 +133,7 @@ int scatter_typed(const float* src, const void* index_, float* out, float* count
     if (reduce == B200MP_MAX) init = -__builtin_inff();
     if (reduce == B200MP_MUL) init = 1.0f;
     unsigned fb = blocks_for(n_out);
-    if (fb > 148u * 16u) fb = 148u * 16u;
+    if (fb > static_cast<unsigned>(num_sms()) * 16u) fb = static_cast<unsigned>(num_sms()) * 16u;
     if (init == 0.0f) B200MP_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * n_out, s));
     else fill_f32_kernel<<<fb, kT, 0, s>>>(out, n_out, init);
     if (need_count) B200MP_CUDA(cudaMemsetAsync(count, 0, sizeof(float) * n_rows, s));

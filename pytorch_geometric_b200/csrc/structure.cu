@@ -355,7 +355,7 @@ extern "C" int b200mp_index_stats(const void* index, int64_t n_index, int64_t* s
     if (n_index > 0) {
         B200MP_CHECK_ARG(index);
         int64_t blocks = ceil_div(n_index, kThreads);
-        if (blocks > 148 * 8) blocks = 148 * 8;
+        if (blocks > num_sms() * 8) blocks = num_sms() * 8;
         IDX_DISPATCH((index_stats_kernel<int32_t><<<static_cast<unsigned>(blocks), kThreads, 0, s>>>(static_cast<const int32_t*>(index), n_index, st)),
                      (index_stats_kernel<int64_t><<<static_cast<unsigned>(blocks), kThreads, 0, s>>>(static_cast<const int64_t*>(index), n_index, st)));
     }

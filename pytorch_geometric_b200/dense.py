@@ -1,7 +1,7 @@
 """The layer's dense transform `x W^T (+ b)` (reference: nn/dense/linear.py:121-127, F.linear).
 
 Two back ends, same fp32-level accuracy:
-  * "tf32x3" (default on shapes it supports): the hand-written tcgen05/TMEM/TMA 3xTF32 GEMMs of
+  * "tf32x3" (default on shapes it supports): the hand-written wgmma/TMA 3xTF32 GEMMs of
     csrc/gemm_tf32x3.cu -- forward, grad-input and the split-K grad-weight product all read x, g
     and W exactly as they lie in HBM;
   * "cublas": torch.nn.functional.linear in strict fp32 (what the reference runs) -- used for
@@ -21,7 +21,7 @@ from . import ops
 from ._lib import check, lib
 
 _BACKEND = "tf32x3"
-DEFAULT_GEMM_MODE = 1   # library default of b200mp_set_option("gemm_mode"): 0 = SS, 1 = TS (A operand in TMEM)
+DEFAULT_GEMM_MODE = 1   # library default of b200mp_set_option("gemm_mode") (accepted; the sm_90a kernel has one configuration)
 DEFAULT_GEMM_PREFETCH = 0   # library default of b200mp_set_option("gemm_prefetch") (k-blocks ahead, 0 = off)
 _B_SPLIT = False            # True: pass W unsplit and let the kernel split its B tiles (w_lo == NULL in the C ABI)
 
@@ -116,7 +116,7 @@ def linear_grad_weight(g: Tensor, x: Tensor) -> Tensor:
 
 def gemm_pair(a1: Tensor, a2: Optional[Tensor], b_hi: Tensor, b_lo: Optional[Tensor], b_layout: int, n1: int, n2: int = 0,
               bias: Optional[Tensor] = None, relu: bool = False, out1: Optional[Tensor] = None):
-    """[c1 | c2] = act([a1 | a2] . B + bias) on the TS-mode tcgen05 kernel (b200mp_gemm_pair_tf32x3)."""
+    """[c1 | c2] = act([a1 | a2] . B + bias) on the wgmma kernel (b200mp_gemm_pair_tf32x3)."""
     m, k1 = a1.shape
     k2 = 0 if a2 is None else a2.size(1)
     c1 = out1 if out1 is not None else torch.empty((m, n1), dtype=torch.float32, device=a1.device)
@@ -134,7 +134,7 @@ def _pair_ok(x: Tensor, n: int, *ks: int) -> bool:
 
 
 class _LinearTF32x3(torch.autograd.Function):
-    """y = act(x W^T + b): bias (and ReLU) in the GEMM epilogue; backward: mask (ReLU), the two tcgen05 products and a
+    """y = act(x W^T + b): bias (and ReLU) in the GEMM epilogue; backward: mask (ReLU), the two wgmma products and a
     deterministic column sum for the bias."""
 
     @staticmethod
@@ -175,7 +175,7 @@ def linear(x: Tensor, weight: Tensor, bias=None, relu: bool = False) -> Tensor:
 
 
 class _LinearPair(torch.autograd.Function):
-    """y = act(a W_a^T + b W_b^T + bias) in ONE launch (two A streams into one TMEM accumulator); backward: both input
+    """y = act(a W_a^T + b W_b^T + bias) in ONE launch (two A streams into one accumulator); backward: both input
     gradients from one read of g (two outputs of one launch), the weight gradients by the split-K kernel."""
 
     @staticmethod
@@ -261,7 +261,7 @@ def matmul_pair(a: Tensor, w_a: Tensor, b: Tensor, w_b: Tensor, bias: Optional[T
 
 # ---------------------------------------------------------------------------------------------- segment / grouped matmul
 def _mm(a: Tensor, b: Tensor) -> Tensor:
-    """a [M, K] @ b [K, N] (b row-major, as it lies in memory) -- the 3xTF32 tcgen05 kernel where the shape allows."""
+    """a [M, K] @ b [K, N] (b row-major, as it lies in memory) -- the 3xTF32 wgmma kernel where the shape allows."""
     k, n = b.shape
     if (_BACKEND == "tf32x3" and a.is_cuda and a.dtype == torch.float32 and b.dtype == torch.float32 and a.size(0) > 0
             and k % 32 == 0 and _width_ok(n) and a.size(0) < 2**31):
@@ -305,7 +305,7 @@ def _grouped_ok(inputs: Tensor, other: Tensor) -> bool:
 
 
 class _SegmentMatmul(torch.autograd.Function):
-    """Forward and the input gradient are ONE persistent launch each of the grouped tcgen05 kernel (ptr stays on the
+    """Forward and the input gradient are ONE persistent launch each of the grouped wgmma kernel (ptr stays on the
     device); the weight gradient (a reduction over each segment's rows) runs the split-K kernel per segment and reads
     the R + 1 segment bounds to the host once, in the backward only."""
 
@@ -381,7 +381,7 @@ class _SegmentMatmulLoop(torch.autograd.Function):
 def segment_matmul(inputs: Tensor, ptr: Tensor, other: Tensor) -> Tensor:
     """pyg_lib.ops.segment_matmul (nn/dense/linear.py:248-255, nn/conv/rgcn_conv.py:288):
     out[ptr[r]:ptr[r+1]] = inputs[ptr[r]:ptr[r+1]] @ other[r], other: [R, K, N] -- ONE persistent launch of the grouped
-    3xTF32 tcgen05 kernel (fp32-accurate; `ptr` is never read on the host) when K % 32 == 0 and N % 128 == 0, else one
+    3xTF32 wgmma kernel (fp32-accurate; `ptr` is never read on the host) when K % 32 == 0 and N % 128 == 0, else one
     product per segment."""
     if not inputs.is_cuda:
         raise RuntimeError("pytorch_geometric_b200 ops run on CUDA tensors only (no CPU fallback)")

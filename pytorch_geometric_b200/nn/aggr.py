@@ -1,6 +1,6 @@
 """Aggregation modules: mirrors of torch_geometric.nn.aggr.{Sum,Mean,Max,Min,Var,Std,Softmax}Aggregation
 (nn/aggr/base.py:102-185, basic.py:12-50,83-139,142-218), FusedAggregation (fused.py:20-336) and
-MultiAggregation (multi.py:14-200) on the sm_100a kernels.
+MultiAggregation (multi.py:14-200) on the sm_90a kernels.
 
 `__call__(x, index=None, ptr=None, dim_size=None, dim=-2)` has the reference's meaning and error
 behaviour.  Unlike the reference (base.py:177-180 only uses `ptr` in deterministic mode), the CSR

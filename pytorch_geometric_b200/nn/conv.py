@@ -20,7 +20,7 @@ Two layers of code:
 `forward(x, edge_index, ...)` accepts a `[2, E]` tensor or a prebuilt `CSRGraph` -- the counterpart of handing the
 reference a `SparseTensor adj_t`.  Graph structures built from a `[2, E]` tensor are cached by the identity of that
 tensor (`graph.cached_graph`), so a training loop that passes the same edge_index every step sorts once.
-Dense transforms: hand-written tcgen05 3xTF32 GEMMs where the shape allows (dense.py), a library GEMM otherwise.
+Dense transforms: hand-written wgmma 3xTF32 GEMMs where the shape allows (dense.py), a library GEMM otherwise.
 """
 from __future__ import annotations
 
@@ -96,7 +96,7 @@ def gcn_conv(x: Tensor, graph: CSRGraph, weight: Tensor, bias: Optional[Tensor])
 class _SageFused(torch.autograd.Function):
     """One SAGEConv layer on a non-bipartite graph as ONE autograd node (sage_conv.py:120-152):
         agg = aggr_j x_j;  y = act(agg W_l^T + x W_r^T + b)
-    forward  = gather-reduce sweep + one pair GEMM (two A streams into one TMEM accumulator, bias / ReLU in the epilogue);
+    forward  = gather-reduce sweep + one pair GEMM (two A streams into one accumulator, bias / ReLU in the epilogue);
     backward = one pair GEMM for both input gradients (one read of g), the two split-K weight gradients, the bias column
                sum, and the transposed sweep ACCUMULATING into the root gradient (out += A^T g_agg in the kernel epilogue)
     -- no elementwise pass of size N x F exists in either direction except the ReLU mask."""
@@ -304,10 +304,10 @@ def rgcn_conv(x: Tensor, graph: CSRGraph, weight: Tensor, root: Optional[Tensor]
     """RGCNConv with the per-relation semantics of the reference's loop path (rgcn_conv.py:257-280):
     out_i = sum_r aggr_{j in N_r(i)} x_j W_r + x_i root + bias.
 
-    B200 mapping: edges are keyed by the virtual destination `dst * R + r`, so ONE gather-reduce sweep produces
+    Engine mapping: edges are keyed by the virtual destination `dst * R + r`, so ONE gather-reduce sweep produces
     H [N, R*F_in] (per-relation mean/sum for every node) and the R small GEMMs of the reference collapse into ONE
     product with K = R * F_in against [W_1; ...; W_R] (+ the root product accumulated into the same output) -- a true
-    GEMM, on the tcgen05 3xTF32 kernel (no cuBLAS on this path when the widths are supported)."""
+    GEMM, on the wgmma 3xTF32 kernel (no cuBLAS on this path when the widths are supported)."""
     N = x.size(0)
     R, Fi, Fo = weight.shape
     h = Fn.aggregate(graph, x, aggr).view(N, R * Fi)                   # [N*R, F_in] -> [N, R*F_in]
@@ -727,7 +727,7 @@ class TransformerConv(torch.nn.Module):
 
 class HeteroLinear(torch.nn.Module):
     """Mirror of torch_geometric.nn.HeteroLinear (nn/dense/linear.py:174-340): x_k W_k + b_k per type k.  The per-type
-    products are ONE launch of the grouped tcgen05 kernel (dense.segment_matmul); unsorted type vectors are sorted
+    products are ONE launch of the grouped wgmma kernel (dense.segment_matmul); unsorted type vectors are sorted
     with the engine's stable radix sort and the result is un-permuted, as the reference does."""
 
     def __init__(self, in_channels: int, out_channels: int, num_types: int, is_sorted: bool = False, bias: bool = True, **kwargs):

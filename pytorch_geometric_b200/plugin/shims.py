@@ -1,6 +1,6 @@
 """The optional-extension operator signatures the reference binds to (SURVEY.md section 8(b), row 2), served by the
 engine: flipping `torch_geometric.typing.WITH_*` to True with these modules bound makes every `torch_scatter.*`,
-`pyg_lib.ops.*` and `torch.ops.torch_sparse.*` call site of the reference land in the sm_100a kernels.
+`pyg_lib.ops.*` and `torch.ops.torch_sparse.*` call site of the reference land in the sm_90a kernels.
 
   torch_scatter.scatter(src, index, dim, out=None, dim_size=None, reduce=...)      utils/_scatter.py:115,135
   torch_scatter.scatter_max / scatter_min(...) -> (out, arg)                       utils/_scatter.py:156

@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's functional API for the aggregation path: same names,
 argument meaning and error behaviour as torch_geometric.utils.{scatter, segment, softmax, spmm,
-degree, index_sort, add_remaining_self_loops, ...}, routed to the sm_100a kernels.
+degree, index_sort, add_remaining_self_loops, ...}, routed to the sm_90a kernels.
 
 Differences from the reference, all deliberate:
  * CUDA tensors only -- a CPU tensor raises instead of silently running somewhere else.

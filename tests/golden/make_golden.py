@@ -1,8 +1,7 @@
 """Generates tests/golden/*.npz by running the UNMODIFIED reference (pyg-team/pytorch_geometric
-v2.9.0, imported from /root/reference, pure Python over ATen, all WITH_* extension flags False)
-on seeded inputs.  Runs only in the build container (the reference does not exist on the GPU
-box); the .npz files are committed and are what pins the oracle (tests/test_oracle_golden.py)
-and, through it, the CUDA path.
+v2.9.0, installed into oracle/_ref by oracle/install_ref.sh, pure Python over ATen, all WITH_*
+extension flags False) on seeded inputs.  Needs that installed reference; the .npz files are committed
+and are what pins the oracle (tests/test_oracle_golden.py) and, through it, the CUDA path.
 
     python tests/golden/make_golden.py
 
@@ -14,7 +13,7 @@ import sys
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", "oracle", "_ref"))  # oracle/install_ref.sh
 import torch_geometric  # noqa: E402
 import torch_geometric.typing as tgt  # noqa: E402
 from torch_geometric import EdgeIndex  # noqa: E402
@@ -237,7 +236,7 @@ def main():
     save("rgcn", ei=ei, et=et, x=x, R=R, **outs)
 
     with open(os.path.join(OUT, "PROVENANCE.txt"), "w") as f:
-        f.write(f"reference: torch_geometric {torch_geometric.__version__} from /root/reference\n"
+        f.write(f"reference: torch_geometric {torch_geometric.__version__} (unmodified, oracle/install_ref.sh)\n"
                 f"torch: {torch.__version__}\n"
                 f"extensions: WITH_TORCH_SCATTER={tgt.WITH_TORCH_SCATTER} "
                 f"WITH_TORCH_SPARSE={tgt.WITH_TORCH_SPARSE} WITH_PYG_LIB={tgt.WITH_PYG_LIB}\n"

@@ -1,7 +1,7 @@
 """Golden vectors for the multi-aggregation sweep: the UNMODIFIED reference's FusedAggregation
 (torch_geometric/nn/aggr/fused.py) and MultiAggregation (multi.py), forward and backward, on seeded
 inputs with empty groups, ties and constant groups (std mask).  Same provenance rules as make_golden.py
-(runs only in the build container; writes tests/golden/fused_aggr.npz).
+(needs the reference in oracle/_ref; writes tests/golden/fused_aggr.npz).
 
     python tests/golden/make_golden_fused.py
 """
@@ -11,7 +11,7 @@ import sys
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", "oracle", "_ref"))  # oracle/install_ref.sh
 import torch_geometric.typing as tgt  # noqa: E402
 from torch_geometric.nn.aggr import MultiAggregation  # noqa: E402
 from torch_geometric.nn.aggr.fused import FusedAggregation  # noqa: E402

@@ -1,6 +1,6 @@
 """Golden vectors for the next attention row (SURVEY section 8(f) rank 2): the UNMODIFIED reference's GATv2Conv,
-forward and backward, with and without shared weights.  Same provenance rules as make_golden.py (runs only in
-the build container; writes tests/golden/gatv2.npz).
+forward and backward, with and without shared weights.  Same provenance rules as make_golden.py (needs the
+reference in oracle/_ref; writes tests/golden/gatv2.npz).
 
     python tests/golden/make_golden_gatv2.py
 """
@@ -10,7 +10,7 @@ import sys
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", "oracle", "_ref"))  # oracle/install_ref.sh
 import torch_geometric.typing as tgt  # noqa: E402
 from torch_geometric.nn import GATv2Conv  # noqa: E402
 

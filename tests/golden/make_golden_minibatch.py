@@ -1,7 +1,7 @@
 """Golden vectors for the mini-batch side (SURVEY section 8(f) rank 4) from the UNMODIFIED reference:
 `trim_to_layer` driving a 3-layer SAGE model over a BFS-ordered sampled subgraph (the layout NeighborLoader emits:
 hops concatenated, each hop grouped by destination), and `coalesce` with duplicates and every reduce.
-Same provenance rules as make_golden.py (runs only in the build container; writes tests/golden/minibatch.npz).
+Same provenance rules as make_golden.py (needs the reference in oracle/_ref; writes tests/golden/minibatch.npz).
 
     python tests/golden/make_golden_minibatch.py
 """
@@ -11,7 +11,7 @@ import sys
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", "oracle", "_ref"))  # oracle/install_ref.sh
 import torch_geometric.typing as tgt  # noqa: E402
 from torch_geometric.nn import SAGEConv  # noqa: E402
 from torch_geometric.utils import coalesce, trim_to_layer  # noqa: E402

@@ -55,26 +55,38 @@ def test_state_dict_layout_matches_reference_layers():
     assert sd["weight"].shape == (3, 8, 16) and sd["root"].shape == (8, 16) and sd["bias"].shape == (16, )
 
 
-def test_state_dict_names_and_shapes_equal_the_reference_layers(tg):
-    """Checkpoints are interchangeable: same keys AND shapes as the reference's layers, option by option (GIN's eps is [1],
-    `edge_dim` adds `lin_edge` / `att_edge`, `share_weights` registers one module under two names, ...)."""
-    import pytorch_geometric_b200.nn as ours
+def STATE_DICT_CASES():
     mlp = lambda: torch.nn.Sequential(torch.nn.Linear(8, 16), torch.nn.ReLU(), torch.nn.Linear(16, 16))   # noqa: E731
-    cases = [("GCNConv", (8, 16), {}), ("SAGEConv", (8, 16), {}), ("SAGEConv", (8, 16), {"project": True}),
-             ("GATConv", (8, 4), {"heads": 3}), ("GATConv", (8, 4), {"heads": 2, "concat": False, "residual": True}),
-             ("RGCNConv", (8, 16, 3), {}), ("GINConv", (mlp(), ), {"train_eps": True}), ("GINConv", (mlp(), ), {}),
-             ("GATConv", (8, 4), {"heads": 2, "edge_dim": 3}), ("GATConv", ((8, 6), 4), {"heads": 2}),
-             ("GATv2Conv", (8, 4), {"heads": 3, "edge_dim": 5}),
-             ("GATv2Conv", (8, 4), {"heads": 2, "share_weights": True, "residual": True, "concat": False}),
-             ("TransformerConv", (8, 4), {"heads": 3, "edge_dim": 5, "beta": True}),
-             ("TransformerConv", (8, 4), {"heads": 2, "concat": False, "bias": False}),
-             ("GraphConv", (8, 16), {}), ("RGCNConv", (8, 16, 3), {"num_bases": 2}), ("RGCNConv", (8, 16, 3), {"num_blocks": 4}),
-             ("FastRGCNConv", (8, 16, 3), {}), ("HeteroLinear", (8, 16, 3), {}), ("HeteroLinear", (8, 16, 3), {"bias": False})]
-    for name, args, kw in cases:
+    return [("GCNConv", (8, 16), {}), ("SAGEConv", (8, 16), {}), ("SAGEConv", (8, 16), {"project": True}),
+            ("GATConv", (8, 4), {"heads": 3}), ("GATConv", (8, 4), {"heads": 2, "concat": False, "residual": True}),
+            ("RGCNConv", (8, 16, 3), {}), ("GINConv", (mlp(), ), {"train_eps": True}), ("GINConv", (mlp(), ), {}),
+            ("GATConv", (8, 4), {"heads": 2, "edge_dim": 3}), ("GATConv", ((8, 6), 4), {"heads": 2}),
+            ("GATv2Conv", (8, 4), {"heads": 3, "edge_dim": 5}),
+            ("GATv2Conv", (8, 4), {"heads": 2, "share_weights": True, "residual": True, "concat": False}),
+            ("TransformerConv", (8, 4), {"heads": 3, "edge_dim": 5, "beta": True}),
+            ("TransformerConv", (8, 4), {"heads": 2, "concat": False, "bias": False}),
+            ("GraphConv", (8, 16), {}), ("RGCNConv", (8, 16, 3), {"num_bases": 2}), ("RGCNConv", (8, 16, 3), {"num_blocks": 4}),
+            ("FastRGCNConv", (8, 16, 3), {}), ("HeteroLinear", (8, 16, 3), {}), ("HeteroLinear", (8, 16, 3), {"bias": False})]
+
+
+def test_state_dict_names_and_shapes_equal_the_reference_layers():
+    """Checkpoints are interchangeable: same keys AND shapes as the reference's layers, option by option (GIN's eps is [1],
+    `edge_dim` adds `lin_edge` / `att_edge`, `share_weights` registers one module under two names, ...).  The reference's
+    layouts are stored in tests/golden/state_dict_layout.json (tests/golden/make_golden_reference_api.py)."""
+    import json
+    import os
+
+    import pytorch_geometric_b200.nn as ours
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "state_dict_layout.json")) as f:
+        want = json.load(f)
+    cases = STATE_DICT_CASES()
+    assert len(want) == len(cases)
+    for (name, args, kw), ref in zip(cases, want):
+        assert ref["layer"] == name
         a = getattr(ours, name)(*args, **kw).state_dict()
-        b = getattr(tg.nn, name)(*args, **kw).state_dict()
-        assert {k: tuple(v.shape) for k, v in a.items()} == {k: tuple(v.shape) for k, v in b.items()}, (name, kw)
-        getattr(ours, name)(*args, **kw).load_state_dict(b)          # a reference checkpoint loads
+        assert {k: list(v.shape) for k, v in a.items()} == ref["shapes"], (name, kw)
+        # a reference checkpoint loads (strict: same keys, same shapes)
+        getattr(ours, name)(*args, **kw).load_state_dict({k: torch.zeros(s) for k, s in ref["shapes"].items()})
 
 
 def test_fused_and_multi_aggregation_argument_errors_match_reference_messages():
@@ -116,7 +128,7 @@ def test_multi_aggr_wrapper_rejects_unknown_names_without_a_gpu():
 
 
 def test_prebuilt_library_is_matched_by_content_not_by_file_time():
-    """The .so built here travels to the GPU box in a snapshot whose file times carry no meaning: staleness
+    """A built .so may be copied to another machine with a tree whose file times carry no meaning: staleness
     is decided by a fingerprint of the sources, so touching a file must not trigger minutes of nvcc there."""
     import os
 

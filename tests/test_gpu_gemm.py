@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 3xTF32 dense transform (csrc/gemm_tf32x3.cu) against an fp64
+"""GPU parity of the wgmma 3xTF32 dense transform (csrc/gemm_tf32x3.cu) against an fp64
 reference of the same products: fp32-class accuracy (1e-5 relative to sum |a||b|, the bound an
 fp32 GEMM itself satisfies), ragged row counts, all supported widths, forward and both gradients,
 and the layer-level equivalence with the strict-fp32 library path."""
@@ -23,8 +23,8 @@ def _check(got, ref64, scale64, tol=1e-5):
 
 @pytest.fixture(params=["ss-bk32", "ss-bk16", "ts"])
 def gemm_bk(request):
-    """Kernel variants: SS mode (both operands in shared memory) with 2 x 96 KB or 4 x 48 KB stages,
-    and TS mode (A operand in tensor memory)."""
+    """Every setting of the GEMM options the library accepts (gemm_mode, gemm_bk, gemm_prefetch) must give the
+    fp32-accurate result; the sm_90a kernel has one configuration, so they must not change it either."""
     from pytorch_geometric_b200 import ops
     ops.set_option("gemm_mode", 1 if request.param == "ts" else 0)
     ops.set_option("gemm_bk", 16 if request.param == "ss-bk16" else 32)
@@ -60,7 +60,7 @@ def test_linear_tf32x3_forward_and_grads(m, n, k, gemm_bk):
 @pytest.mark.parametrize("n,k", [(256, 256), (128, 256), (256, 128), (512, 256)])
 def test_unsplit_weight_gives_the_same_bits(m, n, k):
     """w_lo == NULL: the kernel splits each B tile itself (hi in place, lo next to it).  The split is the same
-    arithmetic, so the results must be bit-identical to the pre-split path (TS mode, both B layouts)."""
+    arithmetic, so the results must be bit-identical to the pre-split path (both B layouts)."""
     from pytorch_geometric_b200 import ops
     ops.set_option("gemm_mode", 1)
     g = torch.Generator(device=DEV).manual_seed(m + n + k)

@@ -189,6 +189,42 @@ int b200mp_minmax_backward(const void* rowptr_t, const void* col_t, const float*
 int b200mp_sddmm_csr(const void* rowptr, const void* col, const void* a, const void* b, float* dot,
                      int64_t n_rows, int64_t feat, int idx_dtype, int val_dtype, void* stream);
 
+/* ------------------------------------------------------------------ edge-feature message relu(x_j + e_ji)
+ * out[i, :] = REDUCE_{e in [rowptr[i], rowptr[i+1])} relu(x[col[e], :] + edge_rows[eid(e), :]), REDUCE = sum | mean,
+ * eid(e) = perm[e] (CSR slot -> caller's edge id; NULL for an adopted CSR whose order is the caller's).
+ * Replaces: GINEConv.message + aggregate (nn/conv/gin_conv.py:195-204 with message_passing.py:263-333,577-595 and
+ * aggr/base.py:173-185): the reference materialises x_j, x_j + edge_attr and its ReLU, three [E, F] tensors.
+ * x: [n_cols, feat], edge_rows: [n_edges, feat] in the caller's edge order (read through perm, never permuted), out:
+ * [n_rows, feat], all val_dtype.  x + edge_rows is rounded to val_dtype before the ReLU (the reference adds in that
+ * dtype); relu(NaN) = NaN; fp32 accumulation in CSR order; mean divides by max(deg, 1); empty rows give 0.
+ * Long rows: plan and partials as in b200mp_spmm_csr.  Every CSR slot belongs to a row (rowptr[n_rows] == n_edges).
+ * mask (nullable: inference) receives the ReLU mask, n_edges * ceil(feat / 8) bytes in CSR order: bit f % 8 of byte
+ * [e * ceil(feat / 8) + f / 8] is set iff !(x + edge_rows <= 0) -- threshold_backward's rule (gradient 0 at 0, passed
+ * through at NaN).  The backward entries below read it. */
+int b200mp_edge_relu_csr(const void* rowptr, const void* col, const void* perm, const void* x,
+                         const void* edge_rows, void* out, void* mask, int64_t n_rows, int64_t n_cols,
+                         int64_t n_edges, int64_t feat, int reduce, const int64_t* long_rows,
+                         const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks, int64_t chunk,
+                         float* partials, int idx_dtype, int val_dtype, void* stream);
+/* grad_x of b200mp_edge_relu_csr over the TRANSPOSED CSR (replaces the index_select backward, an index_add_ with
+ * atomics, and the ReLU backward of gin_conv.py:204):
+ *   grad_x[j, :] = sum_{t in rowT(j)} mask(t2csr[t]) ? val_t[t] * grad_out[col_t[t], :] : 0
+ * t2csr[t] = the CSR slot of transposed slot t; val_t (nullable, fp32) = 1 / max(deg, 1) of the destination for mean.
+ * Long source rows: the transposed CSR's plan and partials. */
+int b200mp_edge_relu_backward_x(const void* rowptr_t, const void* col_t, const void* t2csr,
+                                const float* val_t, const void* grad_out, const void* mask, void* grad_x,
+                                int64_t n_src, int64_t feat, const int64_t* long_rows,
+                                const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks,
+                                int64_t chunk, float* partials, int idx_dtype, int val_dtype, void* stream);
+/* grad_edge_rows of b200mp_edge_relu_csr, in the caller's edge order (the ReLU backward of gin_conv.py:204):
+ *   grad_edge_rows[eid(e), :] = mask(e) ? grad_out[i, :] / (mean ? max(deg_i, 1) : 1) : 0,  e in row i
+ * with the quotient rounded to val_dtype.  Every CSR slot is written once; the plan (no partials) splits hub rows. */
+int b200mp_edge_relu_backward_edge(const void* rowptr, const void* perm, const void* grad_out,
+                                   const void* mask, void* grad_edge_rows, int64_t n_rows, int64_t feat,
+                                   int reduce, const int64_t* long_rows, const int64_t* chunk_ptr,
+                                   int64_t n_long_rows, int64_t n_chunks, int64_t chunk, int idx_dtype,
+                                   int val_dtype, void* stream);
+
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)
  * out[index[e], :] (+)= src[e, :] for an UNSORTED index.  Replaces utils/_scatter.py:14-138
  * (aten::scatter_add_ / scatter_reduce_, torch_scatter.scatter).  fp32 only.  `count` is a

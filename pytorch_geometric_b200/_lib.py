@@ -43,6 +43,9 @@ _SIGS = {
     "b200mp_minmax_ties": (_INT, [_P, _P, _P, _P, _P, _P, _I64, _I64, _INT, _INT, _INT, _P]),
     "b200mp_minmax_backward": (_INT, [_P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _INT, _INT, _P]),
     "b200mp_sddmm_csr": (_INT, [_P, _P, _P, _P, _P, _I64, _I64, _INT, _INT, _P]),
+    "b200mp_edge_relu_csr": (_INT, [_P] * 7 + [_I64] * 4 + [_INT, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
+    "b200mp_edge_relu_backward_x": (_INT, [_P] * 7 + [_I64, _I64, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
+    "b200mp_edge_relu_backward_edge": (_INT, [_P] * 5 + [_I64, _I64, _INT, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
     "b200mp_scatter_coo": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
     "b200mp_split_tf32": (_INT, [_P, _P, _P, _I64, _P]),
     "b200mp_linear_tf32x3": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _P]),

@@ -82,6 +82,57 @@ def aggregate(graph: CSRGraph, x: Tensor, reduce: str = "sum", edge_weight: Opti
     return _Aggregate.apply(x, edge_weight, graph, reduce)
 
 
+class _AggregateEdgeReLU(torch.autograd.Function):
+    """relu(x_j + e_ji) reduced by sum / mean (csrc/edge_relu.cu).  The forward keeps one ReLU bit per (edge, feature)
+    when a gradient is needed; backward = a transposed-CSR sweep for x and, when asked for, a destination sweep that
+    writes the edge-row gradient in the caller's order."""
+
+    @staticmethod
+    def forward(ctx, x: Tensor, edge_rows: Tensor, graph: CSRGraph, reduce: str):
+        want_mask = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
+        out, mask = ops.edge_relu_csr(graph.rowptr, graph.col, graph.perm, x, edge_rows, graph.num_dst, reduce,
+                                      graph.plan, want_mask=want_mask)
+        ctx.graph, ctx.reduce = graph, reduce
+        ctx.save_for_backward(mask)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out: Tensor):
+        mask, = ctx.saved_tensors
+        graph, reduce = ctx.graph, ctx.reduce
+        gx = ga = None
+        if ctx.needs_input_grad[0]:
+            graph.build_transpose()
+            val_t = graph.mean_val_t() if reduce == "mean" else None
+            gx = ops.edge_relu_backward_x(graph.rowptr_t, graph.col_t, graph.t2csr, val_t, grad_out, mask, graph.num_src,
+                                          graph.plan_t)
+        if ctx.needs_input_grad[1]:
+            ga = ops.edge_relu_backward_edge(graph.rowptr, graph.perm, grad_out, mask, graph.num_edges, reduce, graph.plan)
+        return gx, ga, None, None
+
+
+def aggregate_edge_relu(graph: CSRGraph, x: Tensor, edge_rows: Tensor, reduce: str = "sum") -> Tensor:
+    """out[i] = REDUCE_{e = (j -> i)} relu(x[j] + edge_rows[e]) for reduce in {sum, mean}: GINEConv's message and
+    aggregation (gin_conv.py:195-204) without any [E, F] intermediate.  x: [num_src, *], edge_rows: [E, *] with the
+    same trailing shape and dtype, in the caller's edge order; both may require grad.  Empty destinations give 0."""
+    if reduce not in ("sum", "add", "mean"):
+        raise ValueError(f"aggregate_edge_relu reduces by sum or mean, got '{reduce}'")
+    if edge_rows.dtype != x.dtype:
+        raise TypeError(f"edge_rows ({edge_rows.dtype}) and x ({x.dtype}) must share a dtype")
+    if tuple(edge_rows.shape) != (graph.num_edges, ) + tuple(x.shape[1:]):
+        raise ValueError(f"edge_rows must have shape {(graph.num_edges, ) + tuple(x.shape[1:])}, "
+                         f"got {tuple(edge_rows.shape)}")
+    if x.dim() == 1:
+        return aggregate_edge_relu(graph, x.view(-1, 1), edge_rows.view(-1, 1), reduce).view(-1)
+    if x.size(0) != graph.num_src:
+        raise ValueError(f"x has {x.size(0)} rows but the graph has {graph.num_src} source nodes")
+    shape = x.shape[1:]
+    x2 = x.reshape(x.size(0), -1)
+    out = _AggregateEdgeReLU.apply(x2, edge_rows.reshape(graph.num_edges, x2.size(1)), graph,
+                                   "mean" if reduce == "mean" else "sum")
+    return out.view((graph.num_dst, ) + tuple(shape))
+
+
 class _Segment(torch.autograd.Function):
     @staticmethod
     def forward(ctx, src: Tensor, ptr: Tensor, reduce: str):

@@ -11,6 +11,7 @@ Two layers of code:
       SAGEConv        nn/conv/sage_conv.py:19-156        lin_l.weight/bias, lin_r.weight
       GraphConv       nn/conv/graph_conv.py:13-115       lin_rel.weight/bias, lin_root.weight
       GINConv         nn/conv/gin_conv.py:18-105         nn.*, eps [1]
+      GINEConv        nn/conv/gin_conv.py:104-207        nn.*, eps [1], lin.weight/bias (edge_dim)
       RGCNConv        nn/conv/rgcn_conv.py:40-300        weight [R,in,out] (or bases/blocks + comp), root, bias
       FastRGCNConv    nn/conv/rgcn_conv.py:302-374       same parameters
       GATConv         nn/conv/gat_conv.py:27-413         lin (or lin_src/lin_dst), att_src/att_dst, lin_edge/att_edge, res, bias
@@ -453,6 +454,53 @@ class GINConv(torch.nn.Module):
         x = _pair(x)
         graph = _plain_graph(edge_index, x[0].size(0), _num_dst(x, size), self.flow)
         return self.nn(gin_aggregate(x[0], x[1], graph, self.eps))
+
+    def __repr__(self) -> str:
+        return f"{self.__class__.__name__}(nn={self.nn})"
+
+
+class GINEConv(torch.nn.Module):
+    """nn((1 + eps) x_i + AGGR_j relu(x_j + e_ji)) (gin_conv.py:104-207) with AGGR = sum (default) or mean; e_ji =
+    lin(edge_attr) when `edge_dim` is set.  The message and the aggregation run as one edge-feature sweep
+    (`Fn.aggregate_edge_relu`)."""
+
+    def __init__(self, nn: torch.nn.Module, eps: float = 0.0, train_eps: bool = False, edge_dim: Optional[int] = None,
+                 **kwargs):
+        super().__init__()
+        aggr = kwargs.get("aggr", "add")
+        if aggr not in ("add", "sum", "mean"):
+            raise ValueError(f"aggr='{aggr}' is not on the fused path (sum or mean)")
+        self.aggr = "mean" if aggr == "mean" else "sum"
+        self.flow = kwargs.get("flow", "source_to_target")
+        self.nn = nn
+        self.initial_eps = eps
+        if train_eps:
+            self.eps = torch.nn.Parameter(torch.full((1, ), float(eps)))     # shape [1] as gin_conv.py:146-149
+        else:
+            self.register_buffer("eps", torch.full((1, ), float(eps)))
+        if edge_dim is not None:                                             # gin_conv.py:150-160
+            first = self.nn[0] if isinstance(self.nn, torch.nn.Sequential) else self.nn
+            if hasattr(first, "in_features"):
+                in_channels = first.in_features
+            elif hasattr(first, "in_channels"):
+                in_channels = first.in_channels
+            else:
+                raise ValueError("Could not infer input channels from `nn`.")
+            self.lin = _Lin(edge_dim, in_channels)
+        else:
+            self.lin = None
+
+    def forward(self, x, edge_index: Adj, edge_attr: Optional[Tensor] = None, size=None) -> Tensor:
+        x = _pair(x)
+        if self.lin is None and x[0].size(-1) != edge_attr.size(-1):        # gin_conv.py:197-200
+            raise ValueError("Node and edge feature dimensionalities do not match. Consider setting the 'edge_dim' "
+                             "attribute of 'GINEConv'")
+        graph = _plain_graph(edge_index, x[0].size(0), _num_dst(x, size), self.flow)
+        e = edge_attr if self.lin is None else self.lin(edge_attr)
+        out = Fn.aggregate_edge_relu(graph, x[0], e, self.aggr)
+        if x[1] is not None:
+            out = out + (1 + self.eps) * x[1]
+        return self.nn(out)
 
     def __repr__(self) -> str:
         return f"{self.__class__.__name__}(nn={self.nn})"

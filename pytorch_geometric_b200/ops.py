@@ -377,6 +377,58 @@ def sddmm_csr(rowptr: Tensor, col: Tensor, a: Tensor, b: Tensor) -> Tensor:
     return dot
 
 
+def edge_relu_csr(rowptr: Tensor, col: Tensor, perm: Optional[Tensor], x: Tensor, edge_rows: Tensor, n_rows: int,
+                  reduce: str = "sum", plan: Optional[LongRowPlan] = None,
+                  want_mask: bool = False) -> Tuple[Tensor, Optional[Tensor]]:
+    """out[i,:] = REDUCE_{e in row i} relu(x[col[e],:] + edge_rows[perm[e],:]) for sum / mean, and (want_mask) the
+    ReLU mask, [E, ceil(F / 8)] uint8 bits in CSR order.  edge_rows: [E, F] in the caller's edge order."""
+    _cuda(rowptr, col, perm, x, edge_rows)
+    if reduce not in ("sum", "add", "mean"):
+        raise ValueError(f"edge_relu_csr reduces by sum or mean, not '{reduce}'")
+    x, edge_rows = x.contiguous(), edge_rows.contiguous()
+    E, F = col.numel(), x.size(1)
+    if edge_rows.dtype != x.dtype or tuple(edge_rows.shape) != (E, F):
+        raise ValueError(f"edge_rows must be a [{E}, {F}] tensor of x's dtype, got {tuple(edge_rows.shape)} {edge_rows.dtype}")
+    it = _same_idx(rowptr, col, perm)
+    out = torch.empty(n_rows, F, dtype=x.dtype, device=x.device)
+    mask = torch.empty(E, (F + 7) // 8, dtype=torch.uint8, device=x.device) if want_mask else None
+    pargs, _ = _plan_args(plan, F, x.device)
+    _timed("edge_relu_csr", 2 if pargs[2] else 1, lib().b200mp_edge_relu_csr, _p(rowptr), _p(col), _p(perm), _p(x),
+           _p(edge_rows), _p(out), _p(mask), n_rows, x.size(0), E, F, REDUCE[reduce], *pargs, it, _vdt(x), _stream())
+    return out, mask
+
+
+def edge_relu_backward_x(rowptr_t: Tensor, col_t: Tensor, t2csr: Tensor, val_t: Optional[Tensor], grad_out: Tensor,
+                         mask: Tensor, n_src: int, plan_t: Optional[LongRowPlan] = None) -> Tensor:
+    """grad_x[j,:] = sum_{t in rowT(j)} mask(t2csr[t]) ? val_t[t] * grad_out[col_t[t],:] : 0 (transposed CSR)."""
+    _cuda(rowptr_t, col_t, t2csr, val_t, grad_out, mask)
+    grad_out = grad_out.contiguous()
+    it = _same_idx(rowptr_t, col_t, t2csr)
+    F = grad_out.size(1)
+    grad_x = torch.empty(n_src, F, dtype=grad_out.dtype, device=grad_out.device)
+    pargs, _ = _plan_args(plan_t, F, grad_out.device)
+    _timed("edge_relu_backward_x", 2 if pargs[2] else 1, lib().b200mp_edge_relu_backward_x, _p(rowptr_t), _p(col_t),
+           _p(t2csr), _p(val_t), _p(grad_out), _p(mask), _p(grad_x), n_src, F, *pargs, it, _vdt(grad_out), _stream())
+    return grad_x
+
+
+def edge_relu_backward_edge(rowptr: Tensor, perm: Optional[Tensor], grad_out: Tensor, mask: Tensor, n_edges: int,
+                            reduce: str = "sum", plan: Optional[LongRowPlan] = None) -> Tensor:
+    """grad_edge_rows[perm[e],:] = mask(e) ? grad_out[row(e),:] (/ max(deg, 1) for mean) : 0, caller's edge order."""
+    _cuda(rowptr, perm, grad_out, mask)
+    grad_out = grad_out.contiguous()
+    it = _same_idx(rowptr, perm)
+    F = grad_out.size(1)
+    grad = torch.empty(n_edges, F, dtype=grad_out.dtype, device=grad_out.device)
+    if n_edges == 0:
+        return grad
+    pargs = (_p(plan.long_rows), _p(plan.chunk_ptr), plan.n_long, plan.n_chunks, plan.chunk) \
+        if plan is not None and plan.n_long else (None, None, 0, 0, 0)
+    _timed("edge_relu_backward_edge", 1, lib().b200mp_edge_relu_backward_edge, _p(rowptr), _p(perm), _p(grad_out),
+           _p(mask), _p(grad), rowptr.numel() - 1, F, REDUCE[reduce], *pargs, it, _vdt(grad_out), _stream())
+    return grad
+
+
 def scatter_coo(src: Tensor, index: Tensor, n_rows: int, reduce: str = "sum") -> Tensor:
     """Atomic COO fallback for an unsorted index; fp32, src: [E, F]."""
     _cuda(src, index)

@@ -3,15 +3,22 @@
 
 The reference materialises `x_j = x.index_select(node_dim, edge_index_j)` ([E, F]: 113 GB at the headline shape),
 runs `message` on it and scatters the result.  With the plug-in installed, `_index_select` on a CUDA fp32 / bf16
-feature matrix returns a `LazyRows`: a tensor subclass that only REMEMBERS (matrix, index[, per-edge scale]).
+feature matrix returns a `LazyRows`: a tensor subclass that only REMEMBERS (matrix, index[, per-edge scale]
+[, per-edge rows to add, ReLU]).
 
   * `message` returning `x_j` or `edge_weight.view(-1, 1) * x_j` (GCNConv, SAGEConv, GINConv, GraphConv, ... --
     gcn_conv.py:270-271, graph_conv.py:100-101) keeps it lazy: the multiplication is folded into the scale;
+  * `message` returning `(x_j + edge_attr).relu()` (GINEConv, gin_conv.py:195-204) keeps it lazy too, folded in this
+    order only: first `lazy + t` / `t + lazy` / `torch.add(lazy, t)` (no alpha, no out) with `t` a plain dense
+    tensor of shape [E, *x_j.shape[1:]], x_j's dtype and device, on a lazy without scale; then `relu` (Tensor.relu,
+    torch.relu, F.relu without inplace);
   * `aggregate` -> `Aggregation.reduce` -> `scatter` / `segment` (nn/aggr/base.py:173-185) sees the LazyRows and runs
-    ONE fused gather-reduce over a CSR (`b200mp_spmm_csr`) -- adopted from the sorted `Index`/`ptr` the layer
-    collected, or built by one cached stable sort -- instead of index_select + atomics;
-  * anything else a layer does with `x_j` (concatenation, an MLP, attention logits, ...) materialises it through
-    `__torch_function__` with the very `index_select` the reference would have run, so behaviour is unchanged.
+    ONE fused gather-reduce over a CSR (`b200mp_spmm_csr`, or `b200mp_edge_relu_csr` for the ReLU message, sum / mean)
+    -- adopted from the sorted `Index`/`ptr` the layer collected, or built by one cached stable sort -- instead of
+    index_select + atomics;
+  * anything else a layer does with `x_j` (concatenation, an MLP, attention logits, `* w` after an add, `+ eps` after
+    the ReLU, a min / max reduction, ...) materialises it through `__torch_function__` with the very ops the reference
+    would have run -- index_select, then `+ t`, then relu -- so behaviour, including type promotion, is unchanged.
 
 explain mode and `decomposed_layers > 1` keep working: they call the same `_index_select` / `aggregate`.
 """
@@ -20,6 +27,7 @@ from __future__ import annotations
 from typing import Optional
 
 import torch
+import torch.nn.functional as F
 from torch import Tensor
 
 from ._util import plain
@@ -28,34 +36,44 @@ _META = {"size", "dim", "numel", "stride", "is_floating_point", "is_complex", "i
          "ndimension", "type", "__len__", "is_cuda", "dtype", "device", "shape", "requires_grad", "ndim", "layout", "names",
          "is_sparse", "is_quantized", "is_meta", "grad_fn", "is_leaf", "data_ptr", "_version", "__get__", "__repr__",
          "__format__", "__class__", "__hash__", "__reduce_ex__", "untyped_storage", "storage_offset"}
+_ADD = ("add", "__add__", "__radd__")
 
 
 class LazyRows(Tensor):
-    """rows `index` of `src` along dim 0 (times `scale[e]` per row when set), not yet gathered."""
+    """rows `index` of `src` along dim 0 (times `scale[e]` per row when set; plus `add[e]`, then ReLU'd when `relu`),
+    not yet gathered."""
 
     @staticmethod
-    def __new__(cls, src: Tensor, index: Tensor, scale: Optional[Tensor] = None):
+    def __new__(cls, src: Tensor, index: Tensor, scale: Optional[Tensor] = None, add: Optional[Tensor] = None,
+                relu: bool = False):
         shape = (index.numel(), ) + tuple(src.shape[1:])
         r = Tensor._make_wrapper_subclass(cls, shape, dtype=src.dtype, device=src.device, requires_grad=False)
-        r._src, r._index, r._scale = src, index, scale
+        r._src, r._index, r._scale, r._add, r._relu = src, index, scale, add, relu
         return r
 
     def __repr__(self):                                            # noqa: D105
-        return f"LazyRows(rows={self._index.numel()}, of={tuple(self._src.shape)}, scaled={self._scale is not None})"
+        return (f"LazyRows(rows={self._index.numel()}, of={tuple(self._src.shape)}, scaled={self._scale is not None}, "
+                f"added={self._add is not None}, relu={self._relu})")
 
     def materialise(self) -> Tensor:
-        """What the reference computes: src.index_select(0, index) (* scale)."""
+        """What the reference computes: src.index_select(0, index) (* scale | + add (.relu()))."""
         with torch._C.DisableTorchFunctionSubclass():
             idx = plain(self._index)
             out = self._src.index_select(0, idx)
             if self._scale is not None:
                 s = self._scale
                 out = s.view((-1, ) + (1, ) * (out.dim() - 1)) * out
+            if self._add is not None:
+                out = out + self._add
+                if self._relu:
+                    out = out.relu()
         return out
 
     def _scaled_by(self, w: Tensor) -> Optional["LazyRows"]:
         """self * w for a per-edge weight w of shape [E] / [E, 1, ...]; None when w is anything else."""
         E = self._index.numel()
+        if self._add is not None:
+            return None
         if not isinstance(w, Tensor) or isinstance(w, LazyRows) or w.numel() != E or w.dim() == 0:
             return None
         if w.dim() > 1 and tuple(w.shape) != (E, ) + (1, ) * (w.dim() - 1):
@@ -64,6 +82,16 @@ class LazyRows(Tensor):
             return None
         w1 = w.reshape(-1)
         return LazyRows(self._src, self._index, w1 if self._scale is None else self._scale * w1)
+
+    def _plus(self, t) -> Optional["LazyRows"]:
+        """self + t for per-edge rows t of exactly self's shape, dtype and device; None when t is anything else."""
+        if self._scale is not None or self._add is not None:
+            return None
+        if type(t) is not Tensor or t.layout != torch.strided:
+            return None
+        if tuple(t.shape) != tuple(self.shape) or t.dtype != self.dtype or t.device != self.device:
+            return None
+        return LazyRows(self._src, self._index, add=t)
 
     @classmethod
     def __torch_function__(cls, func, types, args=(), kwargs=None):
@@ -79,7 +107,19 @@ class LazyRows(Tensor):
                 r = lazy._scaled_by(other)
                 if r is not None:
                     return r
-        # anything else: gather now (exactly the reference's index_select) and carry on with a plain tensor
+        if name in _ADD and len(args) == 2 and not kwargs:
+            a, b = args
+            lazy, other = (a, b) if isinstance(a, LazyRows) else (b, a)
+            if isinstance(lazy, LazyRows):
+                r = lazy._plus(other)
+                if r is not None:
+                    return r
+        if (name == "relu" and len(args) == 1 and isinstance(args[0], LazyRows)
+                and (not kwargs or (func is F.relu and kwargs == {"inplace": False}))):
+            lazy = args[0]
+            if lazy._add is not None and not lazy._relu:
+                return LazyRows(lazy._src, lazy._index, add=lazy._add, relu=True)
+        # anything else: gather now (exactly the reference's ops) and carry on with a plain tensor
 
         def mat(v):
             if isinstance(v, LazyRows):

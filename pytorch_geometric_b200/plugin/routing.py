@@ -4,6 +4,10 @@ Every routed function keeps the reference's signature, validation and error mess
 a call iff the feature tensor is a CUDA tensor of dtype float32 / bfloat16 and the reduction is one it implements with
 the reference's semantics; everything else -- CPU tensors, float64 / half / integer data, reduce='any' (whose CUDA result is unspecified in the reference itself) -- falls through to the UNTOUCHED reference function (`__wrapped__`), which is also how the parity oracle
 keeps working next to the engine.  Nothing is ever silently computed on the CPU by the engine.
+
+A `LazyRows` message (lazy.py) meets its destination index in `fused_lazy_reduce`: `x_j` or `w * x_j` becomes one CSR
+gather-reduce (`Fn.aggregate`), `relu(x_j + t)` reduced by sum or mean one edge-feature sweep (`Fn.aggregate_edge_relu`,
+GINEConv's message); any other lazy is materialised by the caller, as the reference would have computed it.
 """
 from __future__ import annotations
 
@@ -54,10 +58,14 @@ def _sorted_ptr(index, dim_size: Optional[int]):
 
 # ------------------------------------------------------------------------------------------------ fused gather + reduce
 def fused_lazy_reduce(lazy: LazyRows, index: Tensor, ptr: Optional[Tensor], dim_size: Optional[int], reduce: str):
-    """aggregate(LazyRows(x, index_j[, w]), index_i) == one CSR gather-reduce; None when not applicable."""
+    """aggregate(LazyRows(x, index_j[, w]), index_i) == one CSR gather-reduce, and
+    aggregate(LazyRows(x, index_j, add=t, relu=True), index_i) == one `relu(x_j + t)` gather-reduce for sum / mean;
+    None when not applicable (the caller then materialises)."""
     r = _REDUCE.get(reduce)
     src = lazy._src
     if r is None or r == "mul" or not engine_ok(src) or index is None:
+        return None
+    if lazy._add is not None and (not lazy._relu or r not in ("sum", "mean")):
         return None
     if lazy._scale is not None and r in ("min", "max") and lazy._scale.requires_grad:
         return None
@@ -66,6 +74,8 @@ def fused_lazy_reduce(lazy: LazyRows, index: Tensor, ptr: Optional[Tensor], dim_
         if dim_size is None:
             return None
     g = graphs.graph_from_pair(lazy._index, index, src.size(0), int(dim_size), ptr=ptr)
+    if lazy._add is not None:
+        return Fn.aggregate_edge_relu(g, src, lazy._add, r)
     x2 = src if src.dim() == 2 else src.reshape(src.size(0), -1)
     w = lazy._scale
     if w is not None and w.dtype != torch.float32:

@@ -225,6 +225,45 @@ int b200mp_edge_relu_backward_edge(const void* rowptr, const void* perm, const v
                                    int64_t n_long_rows, int64_t n_chunks, int64_t chunk, int idx_dtype,
                                    int val_dtype, void* stream);
 
+/* ------------------------------------------------------------------ gated message sigmoid(k_i + q_j) * v_j
+ * out[i, :] = REDUCE_{e in [rowptr[i], rowptr[i+1])} sigmoid(s_e) * v[col[e], :],  s_e = k[i, :] + q[col[e], :],
+ * REDUCE = sum | mean.
+ * Replaces: ResGatedGraphConv.message + aggregate (nn/conv/res_gated_graph_conv.py:128-148 with
+ * message_passing.py:263-333 and aggr/base.py:173-185): the reference materialises k_i, q_j, v_j, their sum, its
+ * sigmoid and the product, six [E, F] tensors.
+ * k: [n_rows, feat]; q, v: [n_cols, feat] rows with a shared row stride `ld` >= feat in elements (two tensors, or the
+ * two halves of one [n_cols, 2 feat] product); out: [n_rows, feat]; all val_dtype.  s_e, sigmoid(s_e) and the product
+ * are each rounded to val_dtype (the reference's add, sigmoid and mul); fp32 accumulation in CSR order; mean divides
+ * by max(deg, 1); empty rows give 0.  Long rows: plan and partials ([n_chunks, feat] fp32) as in b200mp_spmm_csr. */
+int b200mp_gated_csr(const void* rowptr, const void* col, const void* k, const void* q, const void* v,
+                     void* out, int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t feat, int64_t ld,
+                     int reduce, const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows,
+                     int64_t n_chunks, int64_t chunk, float* partials, int idx_dtype, int val_dtype,
+                     void* stream);
+/* grad_k of b200mp_gated_csr over the destination CSR (replaces the autograd of res_gated_graph_conv.py:148 wrt k_i:
+ * mul, sigmoid and add backward, then the index_select backward, an index_add_ with atomics):
+ *   grad_k[i, :] = g_i * sum_{e in row i} v[col[e], :] * sigmoid'(s_e),  g_i = grad_out[i, :] / (mean ? max(deg_i, 1) : 1)
+ * grad_k: [n_rows, feat]; 0 for a row without edges.  Long rows: plan and partials ([n_chunks, feat] fp32). */
+int b200mp_gated_backward_dst(const void* rowptr, const void* col, const void* k, const void* q,
+                              const void* v, const void* grad_out, void* grad_k, int64_t n_rows,
+                              int64_t n_cols, int64_t n_edges, int64_t feat, int64_t ld, int reduce,
+                              const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows,
+                              int64_t n_chunks, int64_t chunk, float* partials, int idx_dtype,
+                              int val_dtype, void* stream);
+/* grad_q and grad_v of b200mp_gated_csr in ONE sweep over the TRANSPOSED CSR (replaces the autograd of
+ * res_gated_graph_conv.py:148 wrt q_j and v_j and its two index_add_ scatters):
+ *   grad_v[j, :] = sum_{t in rowT(j)} sigmoid(s_t) * w_t * grad_out[col_t[t], :]
+ *   grad_q[j, :] = v[j, :] * sum_{t in rowT(j)} sigmoid'(s_t) * w_t * grad_out[col_t[t], :]
+ * s_t = k[col_t[t], :] + q[j, :] rounded to val_dtype; w_t = val_t[t] (nullable, fp32: 1 / max(deg, 1) of the
+ * destination for mean) or 1.  grad_q, grad_v: [n_src, feat] rows with q's and v's stride `ld`; 0 for a source
+ * without out-edges.  Long source rows: the transposed CSR's plan, partials [n_chunks, 2 feat] fp32. */
+int b200mp_gated_backward_src(const void* rowptr_t, const void* col_t, const float* val_t, const void* k,
+                              const void* q, const void* v, const void* grad_out, void* grad_q,
+                              void* grad_v, int64_t n_src, int64_t n_dst, int64_t n_edges, int64_t feat,
+                              int64_t ld, const int64_t* long_rows, const int64_t* chunk_ptr,
+                              int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials,
+                              int idx_dtype, int val_dtype, void* stream);
+
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)
  * out[index[e], :] (+)= src[e, :] for an UNSORTED index.  Replaces utils/_scatter.py:14-138
  * (aten::scatter_add_ / scatter_reduce_, torch_scatter.scatter).  fp32 only.  `count` is a

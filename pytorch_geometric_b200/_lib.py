@@ -46,6 +46,9 @@ _SIGS = {
     "b200mp_edge_relu_csr": (_INT, [_P] * 7 + [_I64] * 4 + [_INT, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
     "b200mp_edge_relu_backward_x": (_INT, [_P] * 7 + [_I64, _I64, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
     "b200mp_edge_relu_backward_edge": (_INT, [_P] * 5 + [_I64, _I64, _INT, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
+    "b200mp_gated_csr": (_INT, [_P] * 6 + [_I64] * 5 + [_INT, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
+    "b200mp_gated_backward_dst": (_INT, [_P] * 7 + [_I64] * 5 + [_INT, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
+    "b200mp_gated_backward_src": (_INT, [_P] * 9 + [_I64] * 5 + [_P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
     "b200mp_scatter_coo": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
     "b200mp_split_tf32": (_INT, [_P, _P, _P, _I64, _P]),
     "b200mp_linear_tf32x3": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _P]),

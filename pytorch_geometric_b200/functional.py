@@ -133,6 +133,79 @@ def aggregate_edge_relu(graph: CSRGraph, x: Tensor, edge_rows: Tensor, reduce: s
     return out.view((graph.num_dst, ) + tuple(shape))
 
 
+class _AggregateGated(torch.autograd.Function):
+    """sigmoid(k_i + q_j) * v_j reduced by sum / mean (csrc/gated.cu).  Nothing per edge is saved: the backward
+    recomputes the gate from k and q.  grad_k is a destination sweep, grad_q and grad_v one transposed-CSR sweep; each
+    runs only when one of its inputs needs a gradient.  `v` None means `q` is one [N, 2F] tensor holding q | v."""
+
+    @staticmethod
+    def forward(ctx, k: Tensor, q: Tensor, v: Optional[Tensor], graph: CSRGraph, reduce: str):
+        F = k.size(1)
+        qq, vv = (q, v) if v is not None else (q[:, :F], q[:, F:])
+        out = ops.gated_csr(graph.rowptr, graph.col, k, qq, vv, graph.num_dst, reduce, graph.plan)
+        ctx.graph, ctx.reduce, ctx.split = graph, reduce, v is None
+        ctx.save_for_backward(k, q, v)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out: Tensor):
+        k, q, v = ctx.saved_tensors
+        graph, reduce = ctx.graph, ctx.reduce
+        F = k.size(1)
+        qq, vv = (q[:, :F], q[:, F:]) if ctx.split else (q, v)
+        gk = gq = gv = None
+        if ctx.needs_input_grad[0]:
+            gk = ops.gated_backward_dst(graph.rowptr, graph.col, k, qq, vv, grad_out, reduce, graph.plan)
+        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            graph.build_transpose()
+            val_t = graph.mean_val_t() if reduce == "mean" else None
+            gq = torch.empty_like(q)
+            gv = None if ctx.split else torch.empty_like(v)
+            ops.gated_backward_src(graph.rowptr_t, graph.col_t, val_t, k, qq, vv, grad_out,
+                                   gq[:, :F] if ctx.split else gq, gq[:, F:] if ctx.split else gv, graph.plan_t)
+        return gk, gq, gv, None, None
+
+
+def _gated_check(graph: CSRGraph, k: Tensor, q: Tensor, reduce: str, name: str) -> None:
+    if reduce not in ("sum", "add", "mean"):
+        raise ValueError(f"{name} reduces by sum or mean, got '{reduce}'")
+    if q.dtype != k.dtype:
+        raise TypeError(f"q ({q.dtype}) and k ({k.dtype}) must share a dtype")
+    if k.size(0) != graph.num_dst:
+        raise ValueError(f"k has {k.size(0)} rows but the graph has {graph.num_dst} destination nodes")
+    if q.size(0) != graph.num_src:
+        raise ValueError(f"q has {q.size(0)} rows but the graph has {graph.num_src} source nodes")
+
+
+def aggregate_gated(graph: CSRGraph, k: Tensor, q: Tensor, v: Tensor, reduce: str = "sum") -> Tensor:
+    """out[i] = REDUCE_{e = (j -> i)} sigmoid(k[i] + q[j]) * v[j] for reduce in {sum, mean}: ResGatedGraphConv's
+    message and aggregation (res_gated_graph_conv.py:138-148) without any [E, F] intermediate.  k: [num_dst, *];
+    q, v: [num_src, *] with k's trailing shape and dtype; all three may require grad.  Empty destinations give 0."""
+    _gated_check(graph, k, q, reduce, "aggregate_gated")
+    if v.dtype != k.dtype:
+        raise TypeError(f"v ({v.dtype}) and k ({k.dtype}) must share a dtype")
+    if q.shape[1:] != k.shape[1:] or v.shape != q.shape:
+        raise ValueError(f"q and v must have shape {(graph.num_src, ) + tuple(k.shape[1:])}, "
+                         f"got {tuple(q.shape)} and {tuple(v.shape)}")
+    if k.dim() == 1:
+        return aggregate_gated(graph, k.view(-1, 1), q.view(-1, 1), v.view(-1, 1), reduce).view(-1)
+    shape = k.shape[1:]
+    k2 = k.reshape(k.size(0), -1).contiguous()
+    q2 = q.reshape(q.size(0), -1).contiguous()
+    v2 = v.reshape(v.size(0), -1).contiguous()
+    out = _AggregateGated.apply(k2, q2, v2, graph, "mean" if reduce == "mean" else "sum")
+    return out.view((graph.num_dst, ) + tuple(shape))
+
+
+def aggregate_gated_qv(graph: CSRGraph, k: Tensor, qv: Tensor, reduce: str = "sum") -> Tensor:
+    """aggregate_gated with q and v as the two halves of one [num_src, 2F] tensor (one product with the concatenated
+    query / value weights), read in place; its gradient is one [num_src, 2F] tensor as well.  k: [num_dst, F]."""
+    _gated_check(graph, k, qv, reduce, "aggregate_gated_qv")
+    if k.dim() != 2 or qv.dim() != 2 or qv.size(1) != 2 * k.size(1):
+        raise ValueError(f"k must be [num_dst, F] and qv [num_src, 2F], got {tuple(k.shape)} and {tuple(qv.shape)}")
+    return _AggregateGated.apply(k.contiguous(), qv.contiguous(), None, graph, "mean" if reduce == "mean" else "sum")
+
+
 class _Segment(torch.autograd.Function):
     @staticmethod
     def forward(ctx, src: Tensor, ptr: Tensor, reduce: str):

@@ -12,6 +12,7 @@ Two layers of code:
       GraphConv       nn/conv/graph_conv.py:13-115       lin_rel.weight/bias, lin_root.weight
       GINConv         nn/conv/gin_conv.py:18-105         nn.*, eps [1]
       GINEConv        nn/conv/gin_conv.py:104-207        nn.*, eps [1], lin.weight/bias (edge_dim)
+      ResGatedGraphConv nn/conv/res_gated_graph_conv.py:13-148  lin_key/lin_query/lin_value.weight/bias, lin_skip.weight, bias
       RGCNConv        nn/conv/rgcn_conv.py:40-300        weight [R,in,out] (or bases/blocks + comp), root, bias
       FastRGCNConv    nn/conv/rgcn_conv.py:302-374       same parameters
       GATConv         nn/conv/gat_conv.py:27-413         lin (or lin_src/lin_dst), att_src/att_dst, lin_edge/att_edge, res, bias
@@ -504,6 +505,52 @@ class GINEConv(torch.nn.Module):
 
     def __repr__(self) -> str:
         return f"{self.__class__.__name__}(nn={self.nn})"
+
+
+class ResGatedGraphConv(torch.nn.Module):
+    """W_1 x_i + AGGR_j sigmoid(W_3 x_i + W_4 x_j) * W_2 x_j (+ bias) (res_gated_graph_conv.py:13-148) with AGGR = sum
+    (default) or mean.  q | v come from one product with the concatenated query / value weights, and the gated
+    message runs with its aggregation as one sweep (`Fn.aggregate_gated_qv`).  `edge_dim` and gates other than the
+    sigmoid are not on the fused path and raise ValueError."""
+
+    def __init__(self, in_channels, out_channels: int, act=torch.nn.Sigmoid(), edge_dim: Optional[int] = None,
+                 root_weight: bool = True, bias: bool = True, **kwargs):
+        super().__init__()
+        aggr = kwargs.get("aggr", "add")
+        if aggr not in ("add", "sum", "mean"):
+            raise ValueError(f"aggr='{aggr}' is not on the fused path (sum or mean)")
+        if edge_dim is not None:
+            raise ValueError("edge_dim is not on the fused path (the gate would need per-edge Linear inputs)")
+        if not (isinstance(act, torch.nn.Sigmoid) or act in (torch.sigmoid, F.sigmoid)):
+            raise ValueError(f"act={act!r} is not on the fused path (only the sigmoid gate is)")
+        self.aggr = "mean" if aggr == "mean" else "sum"
+        self.flow = kwargs.get("flow", "source_to_target")
+        self.in_channels, self.out_channels = in_channels, out_channels
+        self.act, self.edge_dim, self.root_weight = act, edge_dim, root_weight
+        ic = (in_channels, in_channels) if isinstance(in_channels, int) else tuple(in_channels)
+        self.lin_key = _Lin(ic[1], out_channels)                            # res_gated_graph_conv.py:80-93
+        self.lin_query = _Lin(ic[0], out_channels)
+        self.lin_value = _Lin(ic[0], out_channels)
+        self.lin_skip = _Lin(ic[1], out_channels, bias=False) if root_weight else None
+        self.bias = torch.nn.Parameter(torch.zeros(out_channels)) if bias else None
+
+    def forward(self, x, edge_index: Adj, edge_attr: Optional[Tensor] = None) -> Tensor:
+        assert edge_attr is None                                             # res_gated_graph_conv.py:141
+        x = _pair(x)
+        k = self.lin_key(x[1])
+        w_qv = torch.cat([self.lin_query.weight, self.lin_value.weight], dim=0)
+        b_qv = torch.cat([self.lin_query.bias, self.lin_value.bias], dim=0)
+        qv = dense.linear(x[0], w_qv, b_qv)
+        graph = _plain_graph(edge_index, x[0].size(0), x[1].size(0), self.flow)
+        out = Fn.aggregate_gated_qv(graph, k, qv, self.aggr)
+        if self.lin_skip is not None:
+            out = out + self.lin_skip(x[1])
+        if self.bias is not None:
+            out = out + self.bias
+        return out
+
+    def __repr__(self) -> str:
+        return f"{self.__class__.__name__}({self.in_channels}, {self.out_channels})"
 
 
 class RGCNConv(torch.nn.Module):

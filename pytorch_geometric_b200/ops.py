@@ -429,6 +429,74 @@ def edge_relu_backward_edge(rowptr: Tensor, perm: Optional[Tensor], grad_out: Te
     return grad
 
 
+def _gated_rows(k: Tensor, q: Tensor, v: Tensor) -> int:
+    """Check the operands of the gated sweeps; returns the row stride `ld` that q and v (and their gradients) share."""
+    F = k.size(1)
+    if k.dim() != 2 or not k.is_contiguous():
+        raise ValueError("k must be a contiguous 2-D tensor")
+    for name, t in (("q", q), ("v", v)):
+        if t.dim() != 2 or t.size(1) != F or t.dtype != k.dtype or (t.size(0) > 0 and t.stride(1) != 1):
+            raise ValueError(f"{name} must be a [N, {F}] tensor of k's dtype with unit feature stride, "
+                             f"got {tuple(t.shape)} {t.dtype}")
+    if q.size(0) != v.size(0) or q.stride(0) != v.stride(0) or q.stride(0) < F:
+        raise ValueError(f"q and v must have the same rows and one row stride >= {F}, got strides "
+                         f"{q.stride()} and {v.stride()}")
+    return q.stride(0)
+
+
+def gated_csr(rowptr: Tensor, col: Tensor, k: Tensor, q: Tensor, v: Tensor, n_rows: int, reduce: str = "sum",
+              plan: Optional[LongRowPlan] = None) -> Tensor:
+    """out[i,:] = REDUCE_{e in row i} sigmoid(k[i,:] + q[col[e],:]) * v[col[e],:] for sum / mean.  k: [n_rows, F]
+    contiguous; q, v: [n_src, F] rows sharing one row stride (two tensors, or the halves of one [n_src, 2F])."""
+    _cuda(rowptr, col, k, q, v)
+    if reduce not in ("sum", "add", "mean"):
+        raise ValueError(f"gated_csr reduces by sum or mean, not '{reduce}'")
+    ld = _gated_rows(k, q, v)
+    it = _same_idx(rowptr, col)
+    F = k.size(1)
+    out = torch.empty(n_rows, F, dtype=k.dtype, device=k.device)
+    pargs, _ = _plan_args(plan, F, k.device)
+    _timed("gated_csr", 2 if pargs[2] else 1, lib().b200mp_gated_csr, _p(rowptr), _p(col), _p(k), _p(q), _p(v),
+           _p(out), n_rows, q.size(0), col.numel(), F, ld, REDUCE[reduce], *pargs, it, _vdt(k), _stream())
+    return out
+
+
+def gated_backward_dst(rowptr: Tensor, col: Tensor, k: Tensor, q: Tensor, v: Tensor, grad_out: Tensor,
+                       reduce: str = "sum", plan: Optional[LongRowPlan] = None) -> Tensor:
+    """grad_k[i,:] = g_i * sum_{e in row i} v[col[e],:] * sigmoid'(k[i,:] + q[col[e],:]), g_i = grad_out[i,:]
+    (/ max(deg_i, 1) for mean)."""
+    _cuda(rowptr, col, k, q, v, grad_out)
+    ld = _gated_rows(k, q, v)
+    grad_out = grad_out.contiguous()
+    it = _same_idx(rowptr, col)
+    F = k.size(1)
+    grad_k = torch.empty_like(k)
+    pargs, _ = _plan_args(plan, F, k.device)
+    _timed("gated_backward_dst", 2 if pargs[2] else 1, lib().b200mp_gated_backward_dst, _p(rowptr), _p(col), _p(k),
+           _p(q), _p(v), _p(grad_out), _p(grad_k), k.size(0), q.size(0), col.numel(), F, ld, REDUCE[reduce], *pargs,
+           it, _vdt(k), _stream())
+    return grad_k
+
+
+def gated_backward_src(rowptr_t: Tensor, col_t: Tensor, val_t: Optional[Tensor], k: Tensor, q: Tensor, v: Tensor,
+                       grad_out: Tensor, grad_q: Tensor, grad_v: Tensor,
+                       plan_t: Optional[LongRowPlan] = None) -> Tuple[Tensor, Tensor]:
+    """One transposed-CSR sweep writing grad_v[j,:] = sum_t sigmoid(s_t) * w_t g_t and grad_q[j,:] = v[j,:] *
+    sum_t sigmoid'(s_t) * w_t g_t (w_t = val_t[t] or 1) into grad_q / grad_v, which share q's and v's row stride."""
+    _cuda(rowptr_t, col_t, val_t, k, q, v, grad_out, grad_q, grad_v)
+    ld = _gated_rows(k, q, v)
+    if _gated_rows(k, grad_q, grad_v) != ld or grad_q.size(0) != q.size(0):
+        raise ValueError("grad_q and grad_v must have the shape and row stride of q and v")
+    grad_out = grad_out.contiguous()
+    it = _same_idx(rowptr_t, col_t)
+    F = k.size(1)
+    pargs, _ = _plan_args(plan_t, 2 * F, k.device)
+    _timed("gated_backward_src", 2 if pargs[2] else 1, lib().b200mp_gated_backward_src, _p(rowptr_t), _p(col_t),
+           _p(val_t), _p(k), _p(q), _p(v), _p(grad_out), _p(grad_q), _p(grad_v), q.size(0), k.size(0), col_t.numel(),
+           F, ld, *pargs, it, _vdt(k), _stream())
+    return grad_q, grad_v
+
+
 def scatter_coo(src: Tensor, index: Tensor, n_rows: int, reduce: str = "sum") -> Tensor:
     """Atomic COO fallback for an unsorted index; fp32, src: [E, F]."""
     _cuda(src, index)

@@ -12,13 +12,19 @@ feature matrix returns a `LazyRows`: a tensor subclass that only REMEMBERS (matr
     order only: first `lazy + t` / `t + lazy` / `torch.add(lazy, t)` (no alpha, no out) with `t` a plain dense
     tensor of shape [E, *x_j.shape[1:]], x_j's dtype and device, on a lazy without scale; then `relu` (Tensor.relu,
     torch.relu, F.relu without inplace);
+  * `message` returning `act(k_i + q_j) * v_j` with the sigmoid (ResGatedGraphConv, res_gated_graph_conv.py:138-148)
+    becomes a `GatedRows`, folded in this order only: `lazy_a + lazy_b` / `torch.add(lazy_a, lazy_b)` of two plain
+    LazyRows (no scale, no add) of one shape, dtype and device; then `sigmoid` (Tensor.sigmoid, torch.sigmoid,
+    F.sigmoid, nn.Sigmoid -- not `sigmoid_`, not `out=`); then `gate * lazy_v` / `lazy_v * gate` with `lazy_v` a plain
+    LazyRows of the same shape, dtype and device;
   * `aggregate` -> `Aggregation.reduce` -> `scatter` / `segment` (nn/aggr/base.py:173-185) sees the LazyRows and runs
-    ONE fused gather-reduce over a CSR (`b200mp_spmm_csr`, or `b200mp_edge_relu_csr` for the ReLU message, sum / mean)
-    -- adopted from the sorted `Index`/`ptr` the layer collected, or built by one cached stable sort -- instead of
-    index_select + atomics;
+    ONE fused gather-reduce over a CSR (`b200mp_spmm_csr`, or `b200mp_edge_relu_csr` for the ReLU message and
+    `b200mp_gated_csr` for the gated one, sum / mean) -- adopted from the sorted `Index`/`ptr` the layer collected, or
+    built by one cached stable sort -- instead of index_select + atomics;
   * anything else a layer does with `x_j` (concatenation, an MLP, attention logits, `* w` after an add, `+ eps` after
     the ReLU, a min / max reduction, ...) materialises it through `__torch_function__` with the very ops the reference
-    would have run -- index_select, then `+ t`, then relu -- so behaviour, including type promotion, is unchanged.
+    would have run -- index_select, then `+ t`, then relu; or index_select x2, `+`, sigmoid, `*` -- so behaviour,
+    including type promotion, is unchanged.
 
 explain mode and `decomposed_layers > 1` keep working: they call the same `_index_select` / `aggregate`.
 """
@@ -37,6 +43,7 @@ _META = {"size", "dim", "numel", "stride", "is_floating_point", "is_complex", "i
          "is_sparse", "is_quantized", "is_meta", "grad_fn", "is_leaf", "data_ptr", "_version", "__get__", "__repr__",
          "__format__", "__class__", "__hash__", "__reduce_ex__", "untyped_storage", "storage_offset"}
 _ADD = ("add", "__add__", "__radd__")
+_MUL = ("mul", "__mul__", "__rmul__", "multiply")
 
 
 class LazyRows(Tensor):
@@ -100,7 +107,14 @@ class LazyRows(Tensor):
         if name in _META:
             with torch._C.DisableTorchFunctionSubclass():
                 return func(*args, **kwargs)
-        if name in ("mul", "__mul__", "__rmul__", "multiply") and len(args) == 2 and not kwargs:
+        if len(args) == 2 and not kwargs and (name in _ADD or name in _MUL):
+            r = (GatedRows.gate_sum if name in _ADD else GatedRows.gated_message)(*args)
+            if r is not None:
+                return r
+        if (name == "sigmoid" and len(args) == 1 and not kwargs and isinstance(args[0], GatedRows)
+                and args[0]._stage == "sum"):
+            return GatedRows(args[0]._a, args[0]._b, "gate")
+        if name in _MUL and len(args) == 2 and not kwargs:
             a, b = args
             lazy, other = (a, b) if isinstance(a, LazyRows) else (b, a)
             if isinstance(lazy, LazyRows):
@@ -140,3 +154,62 @@ class LazyRows(Tensor):
                 return type(v)(mat(u) for u in v)
             return v
         return func(*mat(args), **{k: mat(v) for k, v in (kwargs or {}).items()})
+
+
+def _plain_lazy(t) -> bool:
+    return type(t) is LazyRows and t._scale is None and t._add is None
+
+
+class GatedRows(LazyRows):
+    """ResGatedGraphConv's message, pending (res_gated_graph_conv.py:148): `a + b` of two plain LazyRows (stage
+    "sum"), its sigmoid ("gate"), then the gate times a plain LazyRows `v` ("message"; `v_first` keeps the operand
+    order).  Still a LazyRows, so every site that materialises a lazy message materialises this one too."""
+
+    @staticmethod
+    def __new__(cls, a: LazyRows, b: LazyRows, stage: str = "sum", v: Optional[LazyRows] = None, v_first: bool = False):
+        r = Tensor._make_wrapper_subclass(cls, a.shape, dtype=a.dtype, device=a.device, requires_grad=False)
+        r._a, r._b, r._stage, r._v, r._v_first = a, b, stage, v, v_first
+        r._scale, r._add, r._relu = None, None, False
+        return r
+
+    def __repr__(self):                                            # noqa: D105
+        return f"GatedRows(rows={self.shape[0]}, stage={self._stage})"
+
+    def materialise(self) -> Tensor:
+        """What the reference computes: a + b (.sigmoid() (* v))."""
+        with torch._C.DisableTorchFunctionSubclass():
+            out = self._a.materialise() + self._b.materialise()
+            if self._stage == "sum":
+                return out
+            out = torch.sigmoid(out)
+            if self._stage == "gate":
+                return out
+            v = self._v.materialise()
+            return v * out if self._v_first else out * v
+
+    def _scaled_by(self, w):
+        return None
+
+    def _plus(self, t):
+        return None
+
+    @staticmethod
+    def gate_sum(a, b) -> Optional["GatedRows"]:
+        """a + b for two plain LazyRows of one shape, dtype and device; None otherwise."""
+        if not (_plain_lazy(a) and _plain_lazy(b)):
+            return None
+        if a.shape != b.shape or a.dtype != b.dtype or a.device != b.device:
+            return None
+        return GatedRows(a, b)
+
+    @staticmethod
+    def gated_message(a, b) -> Optional["GatedRows"]:
+        """gate * v or v * gate for a sigmoid gate and a plain LazyRows v of its shape, dtype and device; None
+        otherwise."""
+        v_first = isinstance(b, GatedRows)
+        gate, v = (b, a) if v_first else (a, b)
+        if not isinstance(gate, GatedRows) or gate._stage != "gate" or not _plain_lazy(v):
+            return None
+        if v.shape != gate.shape or v.dtype != gate.dtype or v.device != gate.device:
+            return None
+        return GatedRows(gate._a, gate._b, "message", v, v_first)

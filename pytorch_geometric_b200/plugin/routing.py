@@ -7,7 +7,8 @@ keeps working next to the engine.  Nothing is ever silently computed on the CPU 
 
 A `LazyRows` message (lazy.py) meets its destination index in `fused_lazy_reduce`: `x_j` or `w * x_j` becomes one CSR
 gather-reduce (`Fn.aggregate`), `relu(x_j + t)` reduced by sum or mean one edge-feature sweep (`Fn.aggregate_edge_relu`,
-GINEConv's message); any other lazy is materialised by the caller, as the reference would have computed it.
+GINEConv's message), `sigmoid(k_i + q_j) * v_j` reduced by sum or mean one gated sweep (`Fn.aggregate_gated`,
+ResGatedGraphConv's message); any other lazy is materialised by the caller, as the reference would have computed it.
 """
 from __future__ import annotations
 
@@ -22,7 +23,7 @@ from .. import utils as U
 from ..graph import CSRGraph
 from . import graphs
 from ._util import plain
-from .lazy import LazyRows
+from .lazy import GatedRows, LazyRows
 
 _ENGINE_DTYPES = (torch.float32, torch.bfloat16)
 _REDUCE = {"sum": "sum", "add": "sum", "mean": "mean", "min": "min", "amin": "min", "max": "max", "amax": "max",
@@ -62,6 +63,8 @@ def fused_lazy_reduce(lazy: LazyRows, index: Tensor, ptr: Optional[Tensor], dim_
     aggregate(LazyRows(x, index_j, add=t, relu=True), index_i) == one `relu(x_j + t)` gather-reduce for sum / mean;
     None when not applicable (the caller then materialises)."""
     r = _REDUCE.get(reduce)
+    if isinstance(lazy, GatedRows):
+        return _fused_gated(lazy, index, ptr, dim_size, r)
     src = lazy._src
     if r is None or r == "mul" or not engine_ok(src) or index is None:
         return None
@@ -82,6 +85,38 @@ def fused_lazy_reduce(lazy: LazyRows, index: Tensor, ptr: Optional[Tensor], dim_
         w = w.float()
     out = Fn.aggregate(g, x2, r, w)
     return out if src.dim() == 2 else out.view((int(dim_size), ) + tuple(src.shape[1:]))
+
+
+def _same_index(a, b) -> bool:
+    """The same index vector: one object, or one data pointer, dtype, shape and stride (`_lift` indexes
+    `edge_index[dim]` afresh for every operand, message_passing.py:321)."""
+    if a is b:
+        return True
+    a, b = _plain(a), _plain(b)
+    return (a.device == b.device and a.dtype == b.dtype and a.shape == b.shape and a.stride() == b.stride()
+            and a.data_ptr() == b.data_ptr())
+
+
+def _fused_gated(lazy: GatedRows, index: Tensor, ptr: Optional[Tensor], dim_size: Optional[int], r: Optional[str]):
+    """aggregate(sigmoid(k_i + q_j) * v_j, index_i) == one gated sweep for sum / mean: the summand gathered by the
+    aggregate's own index is k, the other q, and v must be gathered by q's index.  None otherwise."""
+    if lazy._stage != "message" or r not in ("sum", "mean") or index is None:
+        return None
+    a, b, v = lazy._a, lazy._b, lazy._v
+    a_dst, b_dst = _same_index(a._index, index), _same_index(b._index, index)
+    if a_dst == b_dst:
+        return None
+    k, q = (a, b) if a_dst else (b, a)
+    if not _same_index(v._index, q._index) or not all(engine_ok(t._src) for t in (k, q, v)):
+        return None
+    if dim_size is None:
+        dim_size = getattr(index, "dim_size", None)
+        if dim_size is None:
+            return None
+    if k._src.size(0) != int(dim_size) or v._src.size(0) != q._src.size(0):
+        return None
+    g = graphs.graph_from_pair(q._index, index, q._src.size(0), int(dim_size), ptr=ptr)
+    return Fn.aggregate_gated(g, k._src, q._src, v._src, r)
 
 
 # ------------------------------------------------------------------------------------------------ utils.scatter

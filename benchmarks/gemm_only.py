@@ -37,6 +37,7 @@ def main():
     res = {}
     for name, fn in (("forward", lambda: dense.linear_forward(x, w_hi, w_lo)),
                      ("grad_input", lambda: dense.linear_grad_input(g, w_hi, w_lo)),
+                     ("grad_input_kmajor", lambda: dense.linear_grad_input_w(g, w, w_hi, w_lo)),
                      ("grad_weight", lambda: dense.linear_grad_weight(g, x))):
         for _ in range(2):
             fn()

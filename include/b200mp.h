@@ -491,6 +491,9 @@ int b200mp_attn_csr_backward(int mode, const void* rowptr, const void* col, cons
  * uses a library GEMM): reduction dim % 32 == 0, output width in {64, 128} or a multiple of 256,
  * and for grad_weight N % 128 == 0. */
 int b200mp_split_tf32(const float* w, float* w_hi, float* w_lo, int64_t n, void* stream);
+/* w [rows, cols] -> wt_hi = rn_tf32(w^T), wt_lo = w^T - wt_hi, both [cols, rows]: the input gradient g . w then runs
+ * as the K-major pair form (b_layout 0) on (wt_hi, wt_lo), whose B tiles the kernel reads straight from its TMA stages. */
+int b200mp_split_tf32_transposed(const float* w, float* wt_hi, float* wt_lo, int64_t rows, int64_t cols, void* stream);
 int b200mp_linear_tf32x3(const float* x, const float* w_hi, const float* w_lo, float* y, int64_t m,
                          int64_t n, int64_t k, void* stream);
 int b200mp_linear_grad_input_tf32x3(const float* g, const float* w_hi, const float* w_lo, float* gx,

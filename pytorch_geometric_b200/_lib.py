@@ -51,6 +51,7 @@ _SIGS = {
     "b200mp_gated_backward_src": (_INT, [_P] * 9 + [_I64] * 5 + [_P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
     "b200mp_scatter_coo": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
     "b200mp_split_tf32": (_INT, [_P, _P, _P, _I64, _P]),
+    "b200mp_split_tf32_transposed": (_INT, [_P, _P, _P, _I64, _I64, _P]),
     "b200mp_linear_tf32x3": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _P]),
     "b200mp_linear_grad_input_tf32x3": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _P]),
     "b200mp_linear_grad_weight_workspace_bytes": (_I64, [_I64, _I64, _I64]),

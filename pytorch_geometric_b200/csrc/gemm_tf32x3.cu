@@ -11,18 +11,21 @@
 // accumulated in fp32 registers -- fp32-class accuracy at a third of the TF32 tensor rate.
 //
 // Structure (one persistent CTA per SM, 384 threads = three warpgroups, 128 x BN output tiles, BK = 32):
-//   warpgroup 0     TMA producer: one thread streams the raw fp32 A and B tiles into a 3-deep ring of
-//                   shared-memory stages (cp.async.bulk.tensor.2d, mbarrier complete_tx)
-//   warpgroups 1-2  consumers, 64 output rows each.  Per k-block they
-//                   (1) split the B tile into (hi, lo) K-major 128B-swizzled buffers -- wgmma takes TF32
-//                       operands from shared memory only K-major, so an MN-major B is transposed here;
-//                   (2) load their A fragments straight from the raw tile (either major) into registers and
-//                       split them there: A is the register operand of wgmma, never written back;
-//                   (3) issue 4 k-steps x 3 products of wgmma.m64nBNk8.f32.tf32.tf32 into fp32 registers.
-//                   The epilogue adds the bias, applies ReLU and stores the fragments with masked rows.
+//   warpgroup 0, warp 0   TMA producer: one thread streams the raw fp32 A and B tiles into a ring of shared-memory
+//                         stages (cp.async.bulk.tensor.2d, mbarrier complete_tx)
+//   warpgroup 0, warps 1-3  B preparation, only when B is MN-major or arrives unsplit: split (and transpose) the
+//                         stage's B tile into a 2-slot ring of (hi, lo) K-major 128B-swizzled buffers, one k-block
+//                         ahead of the tensor cores.  A pre-split K-major B (W_hi, W_lo of the forward) is already
+//                         in that layout as TMA writes it: the wgmma descriptors then point at the stage itself.
+//   warpgroups 1-2        consumers, 64 output rows each.  Per k-block they issue 4 k-steps x 3 products of
+//                         wgmma.m64nBNk8.f32.tf32.tf32 (A from registers, B from shared memory) and, while those
+//                         run, load and split the A fragments of the next k-block -- possibly the next tile's --
+//                         into the other of two register sets; then wgmma.wait_group 0, and one thread per
+//                         warpgroup releases the stage (and split slot).  (Keeping a group in flight across
+//                         k-blocks with wait_group 1 made ptxas serialize every wgmma: C7518.)
+//                         The epilogue adds the bias, applies ReLU and stores the fragments with masked rows.
 // Operands may be K-major (row-major [rows, K]) or MN-major (row-major [K, rows]), so all three products
-// read x, g and W exactly as they lie in HBM (no transposes in global memory).  W may arrive pre-split
-// (W_hi, W_lo from b200mp_split_tf32): its two tiles are then copied, not re-split.
+// read x, g and W exactly as they lie in HBM (no transposes in global memory).
 #include <cuda.h>
 
 #include "common.cuh"
@@ -31,9 +34,11 @@ namespace b200mp {
 
 constexpr int kBM = 128;             // output rows per CTA tile (two m64 warpgroups)
 constexpr int kBK = 32;              // fp32 elements of K per stage = one 128-byte swizzle row
-constexpr int kStages = 3;
+constexpr int kMaxStages = 4;
+constexpr int kSplitSlots = 2;       // ring of split B buffers written by the B-preparation warps
+constexpr int kPrepWarps = 3;        // warps 1-3 of warpgroup 0
 constexpr int kGemmThreads = 384;
-constexpr int kConsumerThreads = 256;
+constexpr int kSmemLimit = 227 * 1024;
 constexpr int kMaxSegments = 120;    // grouped form: the tile -> segment table lives in static shared memory
 
 // ---------------------------------------------------------------- PTX wrappers
@@ -65,8 +70,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
         "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
         : "memory");
 }
-// the 256 consumer threads only (named barrier 1; warpgroup 0 never takes part)
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory"); }
 __device__ __forceinline__ float rn_tf32(float a) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(a));
@@ -80,6 +83,17 @@ template <int R>
 __device__ __forceinline__ void fence_regs(float (&d)[R]) {
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// A fragments of one k-block, split: [k-step][register].  Fenced like the accumulators, so that their definitions
+// stay ahead of wgmma.fence and ptxas has no reason to inject warpgroup.arrive inside the MMA window.
+struct AFrag {
+    uint32_t hi[4][4], lo[4][4];
+};
+__device__ __forceinline__ void fence_frag(AFrag& f) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(f.hi[j][i]), "+r"(f.lo[j][i])::"memory");
 }
 
 // d[64 x N] (+)= a[64 x 8] (registers, tf32) . b[8 x N] (shared memory, K-major, tf32)
@@ -174,26 +188,44 @@ __device__ __forceinline__ bool decode_tile(int w, const GemmArgs& args, const i
     return true;
 }
 
+// Shared-memory plan of one instantiation: a ring of raw stages (A tile, then B: raw, or hi and lo when pre-split)
+// and, when B needs preparing, kSplitSlots split (hi, lo) buffers.  As many stages as fit, up to kMaxStages.
+template <int BN, bool B_MN, bool B_PRE>
+struct GemmPlan {
+    static constexpr bool kDirectB = B_PRE && !B_MN;               // wgmma reads B straight from the stage
+    static constexpr uint32_t kABytes = kBM * kBK * 4;             // 16 KB
+    static constexpr uint32_t kBBytes = BN * kBK * 4;
+    static constexpr uint32_t kStageBytes = kABytes + (B_PRE ? 2 : 1) * kBBytes;
+    static constexpr uint32_t kSplitBytes = kDirectB ? 0 : kSplitSlots * 2 * kBBytes;
+    static constexpr uint32_t kFixed = kSplitBytes + 8 * 2 * (kMaxStages + kSplitSlots) + 1024;
+    static constexpr int kFit = static_cast<int>((kSmemLimit - kFixed) / kStageBytes);
+    static constexpr int kStages = kFit < kMaxStages ? kFit : kMaxStages;
+    static constexpr size_t kSmem = kStages * kStageBytes + kFixed;
+    static_assert(kStages >= 2 && kSmem <= kSmemLimit, "one CTA per SM must fit the 227 KB opt-in shared memory of sm_90");
+};
+
 // A_MN / B_MN: operand is MN-major (stored row-major as [K, MN]); B_PRE: B arrives pre-split (tmap_b_hi,
-// tmap_b_lo), else tmap_b_hi is the raw matrix and the consumers split it.
+// tmap_b_lo), else tmap_b_hi is the raw matrix and the B-preparation warps split it.  An MN-major A arrives as
+// four [32 k][32 m] boxes with the 128B swizzle, so the column-wise fragment loads do not collide in one bank.
 template <int BN, bool A_MN, bool B_MN, bool B_PRE, bool GROUPED>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
                    const __grid_constant__ CUtensorMap tmap_b_hi, const __grid_constant__ CUtensorMap tmap_b_lo, GemmArgs args) {
-    constexpr uint32_t kABytes = kBM * kBK * 4;                 // 16 KB
-    constexpr uint32_t kBBytes = BN * kBK * 4;
-    constexpr uint32_t kStageBytes = kABytes + (B_PRE ? 2 : 1) * kBBytes;
-    constexpr uint32_t kTxBytes = kStageBytes;
+    using Plan = GemmPlan<BN, B_MN, B_PRE>;
+    constexpr bool kDirectB = Plan::kDirectB;
+    constexpr int kStages = Plan::kStages;
+    constexpr uint32_t kABytes = Plan::kABytes, kBBytes = Plan::kBBytes, kStageBytes = Plan::kStageBytes;
     constexpr int kAcc = BN / 2;                                // fp32 accumulators per thread (m64 x BN per warpgroup)
 
     extern __shared__ __align__(1024) unsigned char gemm_smem[];
     const uint32_t smem_base = (s2u(gemm_smem) + 1023u) & ~1023u;
     unsigned char* smem_gen = gemm_smem + (smem_base - s2u(gemm_smem));
-    const uint32_t b_hi_buf = smem_base + kStages * kStageBytes;  // split B (K-major, 128B swizzle), shared by both warpgroups
-    const uint32_t b_lo_buf = b_hi_buf + kBBytes;
-    const uint32_t bars = b_lo_buf + kBBytes;
+    const uint32_t split_base = smem_base + kStages * kStageBytes;   // split B slots (K-major, 128B swizzle): hi, lo
+    const uint32_t bars = split_base + Plan::kSplitBytes;
     auto bar_full = [&](int s) { return bars + 8u * s; };
     auto bar_empty = [&](int s) { return bars + 8u * (kStages + s); };
+    auto bar_sfull = [&](int s) { return bars + 8u * (2 * kStages + s); };
+    auto bar_sempty = [&](int s) { return bars + 8u * (2 * kStages + kSplitSlots + s); };
 
     __shared__ int tile_prefix[GROUPED ? kMaxSegments + 2 : 1];
     if (GROUPED && threadIdx.x == 32) {                          // tiles of 128 rows per segment, exclusive prefix
@@ -207,7 +239,11 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     if (threadIdx.x == 0) {
         for (int s = 0; s < kStages; ++s) {
             bar_init(bar_full(s), 1);
-            bar_init(bar_empty(s), kConsumerThreads / 32);       // one arrive per consumer warp
+            bar_init(bar_empty(s), 2 + (kDirectB ? 0 : kPrepWarps));   // one arrive per consumer warpgroup, per prep warp
+        }
+        for (int s = 0; s < kSplitSlots; ++s) {
+            bar_init(bar_sfull(s), kPrepWarps);
+            bar_init(bar_sempty(s), 2);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -215,10 +251,19 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 
     const int n_work = (GROUPED ? tile_prefix[args.n_seg] : args.n_tiles_m) * args.n_tiles_n * args.n_splits;
     const int wg = threadIdx.x >> 7;
+    const int lane = threadIdx.x & 31;
+    auto k_range = [&](const Tile& t, int& kb0, int& kb1) {
+        kb0 = t.split * args.k_blocks_per_split;
+        kb1 = min(kb0 + args.k_blocks_per_split, args.k_blocks);
+    };
 
+    // registers: the producer and B-preparation warpgroup gives up what the two MMA warpgroups need beyond the even
+    // share of 168 (accumulators + two A fragment sets); 128 x 56 + 256 x 224 <= 64 K
     if (wg == 0) {
-        // ===================== TMA producer =====================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 56;" ::: "memory");
+        const int warp = threadIdx.x >> 5;
         if (threadIdx.x == 0) {
+            // ===================== TMA producer =====================
             int stage = 0;
             uint32_t phase = 0;
             for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
@@ -226,16 +271,21 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
                 decode_tile<GROUPED>(w, args, tile_prefix, t);
                 const int m0 = static_cast<int>(t.m0), n0 = t.n0 * BN;
                 const int b_row0 = GROUPED ? t.seg * args.b_seg_rows : 0;       // this segment's block of the stacked B
-                const int kb0 = t.split * args.k_blocks_per_split;
-                const int kb1 = min(kb0 + args.k_blocks_per_split, args.k_blocks);
+                int kb0, kb1;
+                k_range(t, kb0, kb1);
                 for (int kb = kb0; kb < kb1; ++kb) {
                     bar_wait(bar_empty(stage), phase ^ 1u);
                     const uint32_t sa = smem_base + stage * kStageBytes;
                     const uint32_t sb = sa + kABytes;
-                    bar_expect_tx(bar_full(stage), kTxBytes);
-                    if (A_MN) tma_load_2d(sa, &tmap_a, m0, kb * kBK, bar_full(stage));
-                    else if (kb < args.k_blocks_a1) tma_load_2d(sa, &tmap_a, kb * kBK, m0, bar_full(stage));
-                    else tma_load_2d(sa, &tmap_a2, (kb - args.k_blocks_a1) * kBK, m0, bar_full(stage));
+                    bar_expect_tx(bar_full(stage), kStageBytes);
+                    if (A_MN) {
+#pragma unroll
+                        for (int b = 0; b < kBM / 32; ++b) tma_load_2d(sa + b * 4096u, &tmap_a, m0 + 32 * b, kb * kBK, bar_full(stage));
+                    } else if (kb < args.k_blocks_a1) {
+                        tma_load_2d(sa, &tmap_a, kb * kBK, m0, bar_full(stage));
+                    } else {
+                        tma_load_2d(sa, &tmap_a2, (kb - args.k_blocks_a1) * kBK, m0, bar_full(stage));
+                    }
                     if (B_MN) {
                         tma_load_2d(sb, &tmap_b_hi, n0, b_row0 + kb * kBK, bar_full(stage));
                         if (B_PRE) tma_load_2d(sb + kBBytes, &tmap_b_lo, n0, b_row0 + kb * kBK, bar_full(stage));
@@ -246,121 +296,123 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
                     if (++stage == kStages) { stage = 0; phase ^= 1u; }
                 }
             }
+        } else if (!kDirectB && warp >= 1) {
+            // ===================== B preparation: stage -> split slot (hi, lo), K-major 128B swizzle =====================
+            const int pt = threadIdx.x - 32;                    // 0 .. 95
+            int stage = 0, slot = 0;
+            uint32_t phase = 0, sphase = 0;
+            for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
+                Tile t;
+                decode_tile<GROUPED>(w, args, tile_prefix, t);
+                int kb0, kb1;
+                k_range(t, kb0, kb1);
+                for (int kb = kb0; kb < kb1; ++kb) {
+                    bar_wait(bar_full(stage), phase);
+                    bar_wait(bar_sempty(slot), sphase ^ 1u);
+                    const unsigned char* sb = smem_gen + stage * kStageBytes + kABytes;
+                    unsigned char* bh = smem_gen + (split_base - smem_base) + slot * 2 * kBBytes;
+                    unsigned char* bl = bh + kBBytes;
+                    if (!B_MN) {
+                        // raw TMA tile already has the target layout: element-wise
+                        for (uint32_t off = pt * 16u; off < kBBytes; off += kPrepWarps * 32 * 16u) {
+                            const float4 v = *reinterpret_cast<const float4*>(sb + off);
+                            const float4 h = make_float4(rn_tf32(v.x), rn_tf32(v.y), rn_tf32(v.z), rn_tf32(v.w));
+                            *reinterpret_cast<float4*>(bh + off) = h;
+                            *reinterpret_cast<float4*>(bl + off) = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
+                        }
+                    } else {
+                        // raw tile is [32 k][BN n] (unswizzled): gather 4 consecutive k of one n, store one 16-byte chunk
+                        const float* rb = reinterpret_cast<const float*>(sb);
+                        for (int idx = pt; idx < BN * 8; idx += kPrepWarps * 32) {
+                            const int n = idx % BN, kc = idx / BN;
+                            float h[4], l[4];
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) {
+                                const float v = rb[(4 * kc + i) * BN + n];
+                                if (B_PRE) {
+                                    h[i] = v;
+                                    l[i] = rb[BN * kBK + (4 * kc + i) * BN + n];
+                                } else {
+                                    h[i] = rn_tf32(v);
+                                    l[i] = v - h[i];
+                                }
+                            }
+                            const uint32_t off = sw128_offset(n, 4 * kc);
+                            *reinterpret_cast<float4*>(bh + off) = make_float4(h[0], h[1], h[2], h[3]);
+                            *reinterpret_cast<float4*>(bl + off) = make_float4(l[0], l[1], l[2], l[3]);
+                        }
+                    }
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> wgmma (async proxy) reads
+                    __syncwarp();
+                    if (lane == 0) {
+                        bar_arrive(bar_empty(stage));          // this warp has read the raw B of the stage
+                        bar_arrive(bar_sfull(slot));
+                    }
+                    if (++stage == kStages) { stage = 0; phase ^= 1u; }
+                    if (++slot == kSplitSlots) { slot = 0; sphase ^= 1u; }
+                }
+            }
         }
         return;
     }
 
     // ===================== consumers: warpgroups 1 and 2 =====================
-    const int ct = threadIdx.x - 128;                           // 0..255 across both consumer warpgroups
-    const int lane = threadIdx.x & 31;
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;" ::: "memory");
     const int row_base = (wg - 1) * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // fragment rows row_base, +8
     const int kq = lane & 3;
-    int stage = 0;
-    uint32_t phase = 0;
-    float acc[kAcc];
-    for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-        Tile t;
-        decode_tile<GROUPED>(w, args, tile_prefix, t);
-        const int kb0 = t.split * args.k_blocks_per_split;
-        const int kb1 = min(kb0 + args.k_blocks_per_split, args.k_blocks);
+    const bool signal = (threadIdx.x & 127) == 0;               // releases stages / slots for its warpgroup
+    int w = blockIdx.x;
+    if (w >= n_work) return;
+
+    // (A) fragments of this warpgroup's 64 rows from a raw stage, split in registers
+    auto load_a = [&](AFrag& f, int stage) {
+        const unsigned char* sa = smem_gen + stage * kStageBytes;
 #pragma unroll
-        for (int i = 0; i < kAcc; ++i) acc[i] = 0.0f;
-        for (int kb = kb0; kb < kb1; ++kb) {
-            bar_wait(bar_full(stage), phase);
-            const unsigned char* sa = smem_gen + stage * kStageBytes;
-            const unsigned char* sb = sa + kABytes;
-            // (1) B tile -> (hi, lo), K-major 128B swizzle.  Both warpgroups finished their previous wgmmas
-            // (wait_group 0) before this barrier, so the split buffers are free.
-            consumer_sync();
-            unsigned char* bh = smem_gen + (b_hi_buf - smem_base);
-            unsigned char* bl = smem_gen + (b_lo_buf - smem_base);
-            if (!B_MN) {
-                // raw TMA tile already has the target layout: element-wise
+        for (int j = 0; j < kBK / 8; ++j) {
 #pragma unroll
-                for (uint32_t off = ct * 16u; off < kBBytes; off += kConsumerThreads * 16u) {
-                    const float4 v = *reinterpret_cast<const float4*>(sb + off);
-                    float4 h, l;
-                    if (B_PRE) {
-                        h = v;
-                        l = *reinterpret_cast<const float4*>(sb + kBBytes + off);
-                    } else {
-                        h = make_float4(rn_tf32(v.x), rn_tf32(v.y), rn_tf32(v.z), rn_tf32(v.w));
-                        l = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
-                    }
-                    *reinterpret_cast<float4*>(bh + off) = h;
-                    *reinterpret_cast<float4*>(bl + off) = l;
-                }
-            } else {
-                // raw tile is [32 k][BN n] (unswizzled): gather 4 consecutive k of one n, store one 16-byte chunk
-                const float* rb = reinterpret_cast<const float*>(sb);
-#pragma unroll
-                for (int idx = ct; idx < BN * 8; idx += kConsumerThreads) {
-                    const int n = idx % BN, kc = idx / BN;
-                    float v[4], h[4], l[4];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) v[i] = rb[(4 * kc + i) * BN + n];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        if (B_PRE) {
-                            h[i] = v[i];
-                            l[i] = rb[BN * kBK + (4 * kc + i) * BN + n];
-                        } else {
-                            h[i] = rn_tf32(v[i]);
-                            l[i] = v[i] - h[i];
-                        }
-                    }
-                    const uint32_t off = sw128_offset(n, 4 * kc);
-                    *reinterpret_cast<float4*>(bh + off) = make_float4(h[0], h[1], h[2], h[3]);
-                    *reinterpret_cast<float4*>(bl + off) = make_float4(l[0], l[1], l[2], l[3]);
-                }
+            for (int i = 0; i < 4; ++i) {
+                const int r = row_base + (i & 1) * 8, k = j * 8 + kq + (i >> 1) * 4;
+                const float v = A_MN ? *reinterpret_cast<const float*>(sa + (r >> 5) * 4096 + sw128_offset(k, r & 31))
+                                     : *reinterpret_cast<const float*>(sa + sw128_offset(r, k));
+                const float h = rn_tf32(v);
+                f.hi[j][i] = __float_as_uint(h);
+                f.lo[j][i] = __float_as_uint(v - h);
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> wgmma (async proxy) reads
-            // (2) A fragments of this warpgroup's 64 rows, split in registers
-            uint32_t a_hi[kBK / 8][4], a_lo[kBK / 8][4];
-#pragma unroll
-            for (int j = 0; j < kBK / 8; ++j) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int r = row_base + (i & 1) * 8, k = j * 8 + kq + (i >> 1) * 4;
-                    const float v = A_MN ? *reinterpret_cast<const float*>(sa + k * (kBM * 4) + r * 4)
-                                         : *reinterpret_cast<const float*>(sa + sw128_offset(r, k));
-                    const float h = rn_tf32(v);
-                    a_hi[j][i] = __float_as_uint(h);
-                    a_lo[j][i] = __float_as_uint(v - h);
-                }
-            }
-            consumer_sync();                                       // split B visible to both warpgroups
-            __syncwarp();
-            if (lane == 0) bar_arrive(bar_empty(stage));           // raw A and B of this stage are consumed
-            // (3) 4 k-steps x 3 products, small terms first
-            fence_regs(acc);
-            wgmma_fence();
-#pragma unroll
-            for (int j = 0; j < kBK / 8; ++j) {
-                const uint64_t dh = smem_desc_sw128(b_hi_buf + j * 32u);
-                const uint64_t dl = smem_desc_sw128(b_lo_buf + j * 32u);
-                wgmma_tf32<BN>(acc, a_lo[j], dh, (kb > kb0 || j > 0) ? 1u : 0u);
-                wgmma_tf32<BN>(acc, a_hi[j], dl, 1u);
-                wgmma_tf32<BN>(acc, a_hi[j], dh, 1u);
-            }
-            wgmma_commit();
-            wgmma_wait_all();
-            fence_regs(acc);
-            if (++stage == kStages) { stage = 0; phase ^= 1u; }
         }
-        // ===================== epilogue: fragments -> global, rows masked =====================
-        const int nt = t.n0;
+    };
+
+    Tile t;
+    decode_tile<GROUPED>(w, args, tile_prefix, t);
+    int kb0, kb1;
+    k_range(t, kb0, kb1);
+    int kb = kb0;
+    int stage = 0, slot = 0;                                    // ring positions of k-block kb
+    uint32_t phase = 0, sphase = 0;
+    float acc[kAcc];
+    AFrag f0, f1;
+    bar_wait(bar_full(stage), phase);
+    load_a(f0, stage);
+
+    auto release = [&](int st, int sl) {
+        if (signal) {
+            bar_arrive(bar_empty(st));
+            if (!kDirectB) bar_arrive(bar_sempty(sl));
+        }
+    };
+    // epilogue: fragments -> global, rows masked
+    auto store_tile = [&](const Tile& tt) {
+        const int nt = tt.n0;
         const bool second = nt >= args.n_tiles_c1;
         float* out = second ? args.c2 : args.c;
         const int64_t ldc = second ? args.ldc2 : args.ldc;
         const int col0 = (second ? nt - args.n_tiles_c1 : nt) * BN;
         const int bias0 = nt * BN;
-        float* base = out + static_cast<int64_t>(t.split) * args.m * ldc;
+        float* base = out + static_cast<int64_t>(tt.split) * args.m * ldc;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int r = row_base + h * 8;
-            if (r >= t.rows) continue;
-            float* dst = base + (t.m0 + r) * ldc + col0;
+            const bool keep = r < tt.rows;
+            float* dst = base + (tt.m0 + r) * ldc + col0;
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
                 const int c = j * 8 + 2 * kq;
@@ -373,9 +425,60 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
                     v0 = fmaxf(v0, 0.0f);
                     v1 = fmaxf(v1, 0.0f);
                 }
-                *reinterpret_cast<float2*>(dst + c) = make_float2(v0, v1);
+                if (keep) *reinterpret_cast<float2*>(dst + c) = make_float2(v0, v1);
             }
         }
+    };
+    // One k-block: cur holds its A fragments; on return nxt holds those of the next k-block (false: no more work).
+    auto step = [&](AFrag& cur, AFrag& nxt) -> bool {
+        uint32_t b_hi;
+        if (kDirectB) {
+            b_hi = smem_base + stage * kStageBytes + kABytes;
+        } else {
+            bar_wait(bar_sfull(slot), sphase);
+            b_hi = split_base + slot * 2 * kBBytes;
+        }
+        const uint32_t b_lo = b_hi + kBBytes;
+        // 4 k-steps x 3 products, small terms first
+        fence_frag(cur);
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < kBK / 8; ++j) {
+            const uint64_t dh = smem_desc_sw128(b_hi + j * 32u);
+            const uint64_t dl = smem_desc_sw128(b_lo + j * 32u);
+            wgmma_tf32<BN>(acc, cur.lo[j], dh, (kb > kb0 || j > 0) ? 1u : 0u);
+            wgmma_tf32<BN>(acc, cur.hi[j], dl, 1u);
+            wgmma_tf32<BN>(acc, cur.hi[j], dh, 1u);
+        }
+        wgmma_commit();
+        const int cur_stage = stage, cur_slot = slot;
+        if (++stage == kStages) { stage = 0; phase ^= 1u; }
+        if (!kDirectB && ++slot == kSplitSlots) { slot = 0; sphase ^= 1u; }
+        const bool tile_done = ++kb == kb1;
+        Tile tn = t;
+        bool more = true;
+        if (tile_done) {
+            w += gridDim.x;
+            more = w < n_work;
+            if (more) decode_tile<GROUPED>(w, args, tile_prefix, tn);
+        }
+        if (more) {                                             // next A fragments, possibly the next tile's
+            fence_frag(nxt);
+            bar_wait(bar_full(stage), phase);
+            load_a(nxt, stage);
+        }
+        wgmma_wait_all();
+        fence_regs(acc);
+        release(cur_stage, cur_slot);
+        if (tile_done) {
+            store_tile(t);
+            t = tn;
+            k_range(t, kb0, kb1);
+            kb = kb0;
+        }
+        return more;
+    };
+    while (step(f0, f1) && step(f1, f0)) {
     }
 }
 
@@ -386,6 +489,25 @@ __global__ void split_tf32_kernel(const float* __restrict__ w, float* __restrict
         const float v = w[i], h = rn_tf32(v);
         hi[i] = h;
         lo[i] = v - h;
+    }
+}
+// w [rows, cols] -> (rn_tf32(w^T), w^T - rn_tf32(w^T)) [cols, rows], through a 32 x 32 shared-memory tile
+__global__ void split_tf32_transposed_kernel(const float* __restrict__ w, float* __restrict__ hi, float* __restrict__ lo,
+                                             int64_t rows, int64_t cols) {
+    __shared__ float tile[32][33];
+    const int64_t r0 = static_cast<int64_t>(blockIdx.y) * 32, c0 = static_cast<int64_t>(blockIdx.x) * 32;
+    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+        const int64_t r = r0 + i, c = c0 + threadIdx.x;
+        if (r < rows && c < cols) tile[i][threadIdx.x] = w[r * cols + c];
+    }
+    __syncthreads();
+    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+        const int64_t c = c0 + i, r = r0 + threadIdx.x;
+        if (r < rows && c < cols) {
+            const float v = tile[threadIdx.x][i], h = rn_tf32(v);
+            hi[c * rows + r] = h;
+            lo[c * rows + r] = v - h;
+        }
     }
 }
 // out[i] = sum_s part[s][i], fixed order (deterministic split-K)
@@ -415,9 +537,10 @@ static EncodeTiledFn encode_fn() {
 }
 // 2-D fp32 row-major [rows, cols] tensor, zero fill out of bounds.
 //   K-major operand  (mn = false): box = [box_mn rows, 32 cols], 128B swizzle (the wgmma K-major layout);
-//   MN-major operand (mn = true) : box = [32 k-rows, box_mn cols], unswizzled (transposed while it is split).
+//   MN-major operand (mn = true) : box = [32 k-rows, box_mn cols], unswizzled (transposed while it is split),
+//                                  except box_mn = 32 (an MN-major A, loaded as 32-column boxes): 128B swizzle.
 static int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t cols, int64_t ld, bool mn, int box_mn) {
-    const CUtensorMapSwizzle swz = mn ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B;
+    const CUtensorMapSwizzle swz = (mn && box_mn != 32) ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B;
     const int box_cols = mn ? box_mn : kBK;
     const int box_rows = mn ? kBK : box_mn;
     EncodeTiledFn fn = encode_fn();
@@ -446,8 +569,7 @@ static int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t c
 template <int BN, bool A_MN, bool B_MN, bool B_PRE, bool GROUPED = false>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& ta2, const CUtensorMap& tbh, const CUtensorMap& tbl,
                        const GemmArgs& args, int n_work, cudaStream_t stream) {
-    constexpr size_t smem = kStages * (kBM * kBK * 4 + (B_PRE ? 2 : 1) * BN * kBK * 4) + 2 * BN * kBK * 4 + 8 * 2 * kStages + 1024;
-    static_assert(smem <= 227 * 1024, "one CTA per SM must fit the 227 KB opt-in shared memory of sm_90");
+    constexpr size_t smem = GemmPlan<BN, B_MN, B_PRE>::kSmem;
     auto kfn = gemm_tf32x3_kernel<BN, A_MN, B_MN, B_PRE, GROUPED>;
     B200MP_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     const int grid = n_work < num_sms() ? n_work : num_sms();
@@ -518,7 +640,7 @@ static int run_grad_weight(const float* g, const float* x, float* gw, int64_t m,
     }
     CUtensorMap ta, tb;
     int rc;
-    if ((rc = make_map(&ta, g, m, n, n, true, kBM))) return rc;    // A[m' = n-index, k' = row]: stored [K' rows][M' cols]
+    if ((rc = make_map(&ta, g, m, n, n, true, 32))) return rc;     // A[m' = n-index, k' = row]: stored [K' rows][M' cols]
     if ((rc = make_map(&tb, x, m, k, k, true, bn))) return rc;
     GemmArgs args{};
     args.c = static_cast<float*>(workspace);
@@ -546,6 +668,16 @@ extern "C" int b200mp_split_tf32(const float* w, float* w_hi, float* w_lo, int64
     if (n == 0) return B200MP_OK;
     B200MP_CHECK_ARG(w && w_hi && w_lo);
     split_tf32_kernel<<<static_cast<unsigned>(ceil_div(n, 256)), 256, 0, static_cast<cudaStream_t>(stream)>>>(w, w_hi, w_lo, n);
+    B200MP_LAUNCH_CHECK();
+    return B200MP_OK;
+}
+
+extern "C" int b200mp_split_tf32_transposed(const float* w, float* wt_hi, float* wt_lo, int64_t rows, int64_t cols, void* stream) {
+    B200MP_CHECK_ARG(rows >= 0 && cols >= 0);
+    if (rows == 0 || cols == 0) return B200MP_OK;
+    B200MP_CHECK_ARG(w && wt_hi && wt_lo && ceil_div(rows, 32) <= 65535);
+    const dim3 grid(static_cast<unsigned>(ceil_div(cols, 32)), static_cast<unsigned>(ceil_div(rows, 32)));
+    split_tf32_transposed_kernel<<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(w, wt_hi, wt_lo, rows, cols);
     B200MP_LAUNCH_CHECK();
     return B200MP_OK;
 }

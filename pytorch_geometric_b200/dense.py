@@ -65,6 +65,17 @@ def split_tf32(w: Tensor):
     return hi, lo
 
 
+def split_tf32_transposed(w: Tensor):
+    """(rn_tf32(w^T), w^T - rn_tf32(w^T)), both [cols, rows] contiguous."""
+    w = w.detach().contiguous()
+    rows, cols = w.shape
+    hi = torch.empty((cols, rows), dtype=w.dtype, device=w.device)
+    lo = torch.empty_like(hi)
+    ops._timed("split_tf32_transposed", 1, lib().b200mp_split_tf32_transposed, w.data_ptr(), hi.data_ptr(), lo.data_ptr(),
+               rows, cols, ops._stream())
+    return hi, lo
+
+
 def prepare_weight(weight: Tensor):
     """(w_hi, w_lo) for the kernels; (w, None) when the kernel splits B tiles itself."""
     n, k = weight.shape
@@ -93,6 +104,20 @@ def linear_grad_input(g: Tensor, w_hi: Tensor, w_lo: Optional[Tensor]) -> Tensor
     gx = torch.empty((m, k), dtype=torch.float32, device=g.device)
     ops._timed("linear_grad_input_tf32x3", 1, lib().b200mp_linear_grad_input_tf32x3, g.data_ptr(), w_hi.data_ptr(),
                ops._p(w_lo), gx.data_ptr(), m, n, k, ops._stream())
+    return gx
+
+
+def linear_grad_input_w(g: Tensor, weight: Tensor, w_hi: Tensor, w_lo: Optional[Tensor]) -> Tensor:
+    """gx = g W.  Widths that are multiples of 128 split W^T once per call and run the K-major pair form, whose B tiles
+    need no transposing in the kernel; other widths (64) read W MN-major.  Both give the same bits."""
+    m, n = g.shape
+    k = weight.size(1)
+    if k % 128 != 0:
+        return linear_grad_input(g, w_hi, w_lo)
+    wt_hi, wt_lo = split_tf32_transposed(weight)
+    gx = torch.empty((m, k), dtype=torch.float32, device=g.device)
+    ops._timed("linear_grad_input_tf32x3", 1, lib().b200mp_gemm_pair_tf32x3, g.data_ptr(), n, None, 0, wt_hi.data_ptr(),
+               wt_lo.data_ptr(), 0, None, 0, gx.data_ptr(), k, None, 0, m, ops._stream())
     return gx
 
 
@@ -151,16 +176,16 @@ class _LinearTF32x3(torch.autograd.Function):
             if relu:
                 y = y.relu_()
         ctx.relu, ctx.has_bias = relu, bias is not None
-        ctx.save_for_backward(x, w_hi, w_lo, y if relu else None)
+        ctx.save_for_backward(x, weight, w_hi, w_lo, y if relu else None)
         return y
 
     @staticmethod
     def backward(ctx, g: Tensor):
-        x, w_hi, w_lo, y = ctx.saved_tensors
+        x, weight, w_hi, w_lo, y = ctx.saved_tensors
         g = g.contiguous()
         if ctx.relu:
             g = g * (y > 0)
-        gx = linear_grad_input(g, w_hi, w_lo) if ctx.needs_input_grad[0] else None
+        gx = linear_grad_input_w(g, weight, w_hi, w_lo) if ctx.needs_input_grad[0] else None
         gw = linear_grad_weight(g, x) if ctx.needs_input_grad[1] else None
         gb = ops.column_sum(g) if (ctx.has_bias and ctx.needs_input_grad[2]) else None
         return gx, gw, gb, None

@@ -155,7 +155,7 @@ class _LinearInto(torch.autograd.Function):
         x = x.contiguous()
         if dense.get_backend() == "tf32x3" and dense.supported(x, weight):
             w_hi, w_lo = dense.prepare_weight(weight)
-            ctx.save_for_backward(x, w_hi, w_lo)
+            ctx.save_for_backward(x, weight, w_hi, w_lo)
             ctx.fast = True
             dense.linear_forward(x, w_hi, w_lo, out=out)
         else:
@@ -169,8 +169,8 @@ class _LinearInto(torch.autograd.Function):
     def backward(ctx, g: Tensor):
         g = g.contiguous()
         if ctx.fast:
-            x, w_hi, w_lo = ctx.saved_tensors
-            gx = dense.linear_grad_input(g, w_hi, w_lo) if ctx.needs_input_grad[0] else None
+            x, weight, w_hi, w_lo = ctx.saved_tensors
+            gx = dense.linear_grad_input_w(g, weight, w_hi, w_lo) if ctx.needs_input_grad[0] else None
             gw = dense.linear_grad_weight(g, x) if ctx.needs_input_grad[1] else None
         else:
             x, weight = ctx.saved_tensors

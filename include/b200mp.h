@@ -356,6 +356,58 @@ int b200mp_multi_aggr_backward(const void* ptr, const void* idx, const void* x, 
                                void* grad_x, int64_t n_items, int64_t feat, int segment_mode, int idx_dtype,
                                int val_dtype, void* stream);
 
+/* ------------------------------------------------------------------ PNA: shifted multi-aggregation + degree scalers
+ * PNAConv with one pre-layer per tower (nn/conv/pna_conv.py:167-188) sends m_e = u_i + w_e over edge e = (j -> i), with
+ * u = x_t Wa_t^T + b_t, w_e = v_j (+ c_e), v = x_t Wb_t^T, c = edge_encoder(edge_attr) Wc_t^T, all towers side by side
+ * in one width W = towers * feat.  The sweep collects the statistics of w only (b200mp_multi_aggr_csr in gather mode on
+ * v with count_self_zero = 0, or b200mp_pna_edge_stats with edge features); the shift by u, the aggregators and the
+ * scalers are per destination.  Replaces: the message's [E, T, 2F or 3F] concatenation and per-tower Linear
+ * (pna_conv.py:167-188), MultiAggregation's per-aggregator passes over 3-D messages (nn/aggr/multi.py:157), and
+ * DegreeScalerAggregation's degree scatter, per-scaler products and concatenations (nn/aggr/scaler.py:75-109), plus
+ * cat([x, out]) (pna_conv.py:169).
+ * Aggregator codes: 0 sum, 1 mean, 2 min, 3 max, 4 var, 5 std (at most 6); scaler codes: 0 identity, 1 amplification,
+ * 2 attenuation, 3 linear, 4 inverse_linear (at most 5); both lists are host arrays read at the call.
+ * avg_deg_lin / avg_deg_log: device fp32 scalars.  stats_dtype: B200MP_F32 or val_dtype (the statistics' dtype;
+ * ties are fp32).  u: [n_rows, W] rows of stride u_ld; x: [n_rows, W] (x_t of every tower).
+ * Epilogue: out [n_rows, towers, (1 + A S) feat] = cat([x_t, s_1(a_1 .. a_A), .., s_S(a_1 .. a_A)]) per tower, with
+ *   sum = deg u + sum w, mean = sum / max(deg, 1), min / max = u + min / max w (0 for an empty row), var / std from the
+ *   statistics of w (shift-invariant; std clamps at 1e-5 and is zeroed at <= sqrt(1e-5)), deg rounded to val_dtype. */
+int b200mp_pna_epilogue(const void* rowptr, const void* x, const void* u, int64_t u_ld, const void* stat_sum,
+                        const void* stat_min, const void* stat_max, const void* stat_var, const int32_t* aggr_host,
+                        int n_aggr, const int32_t* scaler_host, int n_scaler, const float* avg_deg_lin,
+                        const float* avg_deg_log, void* out, int64_t n_rows, int64_t towers, int64_t feat,
+                        int stats_dtype, int idx_dtype, int val_dtype, void* stream);
+/* Prologue of the backward: folds grad_out (the epilogue's block) into the rows b200mp_multi_aggr_backward or
+ * b200mp_pna_edge_backward read (all nullable, fp32 [n_rows, W]): term_a, term_b, gmin = g_min / ties, gmax = g_max /
+ * ties, where ties count the zero-initialised self of the reference's scatter when the SHIFTED extremum is 0; and in
+ * closed form grad_u (rows of stride gu_ld) = deg g_sum + [deg > 0] g_mean + g_min ties_w_min / ties + g_max ...,
+ * grad_x = the x slot's gradient, avg_part [n_rows, 2] = per-row d L / d avg_deg_lin and d L / d avg_deg_log (the caller
+ * sums the rows in a fixed order). */
+int b200mp_pna_prologue(const void* rowptr, const void* grad_out, const void* u, int64_t u_ld, const void* stat_sum,
+                        const void* stat_min, const void* stat_max, const void* stat_var, const float* ties_min,
+                        const float* ties_max, const int32_t* aggr_host, int n_aggr, const int32_t* scaler_host,
+                        int n_scaler, const float* avg_deg_lin, const float* avg_deg_log, float* term_a, float* term_b,
+                        float* gmin, float* gmax, void* grad_u, int64_t gu_ld, void* grad_x, float* avg_part,
+                        int64_t n_rows, int64_t towers, int64_t feat, int stats_dtype, int idx_dtype, int val_dtype,
+                        void* stream);
+/* Statistics of w_e = v[col[e]] + c[perm[e]] (rounded to val_dtype) over the destination CSR, fp32 [n_rows, width]
+ * planes (each nullable): sum, min, max, var (= sum w^2 / cnt - mean^2), and the tie counts of min / max (no self).
+ * v: [n_cols, width] rows of stride v_ld; c: [n_edges, width] in the caller's edge order, perm: CSR slot -> caller's
+ * edge (nullable = identity).  Hub rows: long-row plan with partials of n_chunks * 6 * width fp32. */
+int b200mp_pna_edge_stats(const void* rowptr, const void* col, const void* perm, const void* v, int64_t v_ld,
+                          const void* c, float* stat_sum, float* stat_min, float* stat_max, float* stat_var,
+                          float* ties_min, float* ties_max, int64_t n_rows, int64_t n_cols, int64_t n_edges,
+                          int64_t width, const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows,
+                          int64_t n_chunks, int64_t chunk, float* partials, int idx_dtype, int val_dtype, void* stream);
+/* Backward of b200mp_pna_edge_stats + the prologue, in ONE sweep over the transposed CSR (rowptr_t, col_t, perm_t =
+ * transposed slot -> caller's edge): d L / d w_e = term_a[i] + w_e term_b[i] + [w_e == min w_i] gmin[i] + [w_e == max
+ * w_i] gmax[i] is written to grad_c[e] and summed into grad_v[j] (rows of stride gv_ld); either output may be null. */
+int b200mp_pna_edge_backward(const void* rowptr_t, const void* col_t, const void* perm_t, const void* v, int64_t v_ld,
+                             const void* c, const float* term_a, const float* term_b, const float* stat_min,
+                             const float* gmin, const float* stat_max, const float* gmax, void* grad_v, int64_t gv_ld,
+                             void* grad_c, int64_t n_src, int64_t n_dst, int64_t n_edges, int64_t width, int idx_dtype,
+                             int val_dtype, void* stream);
+
 /* ------------------------------------------------------------------ node-level attention terms
  * s_a[n,h] = sum_c x[n,h,c] * att_a[h,c] (and s_b with att_b from the same read of x; att_b / s_b nullable together):
  * GATConv's alpha_src / alpha_dst = (x * att).sum(-1) (nn/conv/gat_conv.py:330-331) without the [N,H,C] product tensor.

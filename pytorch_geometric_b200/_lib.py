@@ -85,6 +85,14 @@ _SIGS = {
     "b200mp_head_dot_backward": (_INT, [_P] * 9 + [_I64, _I64, _I64, _I64, _INT, _P]),
     "b200mp_multi_aggr_prepare_backward": (_INT, [_P] * 15 + [_I64, _I64, _INT, _INT, _INT, _P]),
     "b200mp_multi_aggr_backward": (_INT, [_P] * 12 + [_I64, _I64, _INT, _INT, _INT, _P]),
+    "b200mp_pna_epilogue": (_INT, [_P, _P, _P, _I64] + [_P] * 4 + [_P, _INT, _P, _INT, _P, _P, _P, _I64, _I64, _I64,
+                                                                   _INT, _INT, _INT, _P]),
+    "b200mp_pna_prologue": (_INT, [_P, _P, _P, _I64] + [_P] * 6 + [_P, _INT, _P, _INT] + [_P] * 7 + [_I64, _P, _P,
+                                                                                               _I64, _I64, _I64,
+                                                                                               _INT, _INT, _INT, _P]),
+    "b200mp_pna_edge_stats": (_INT, [_P, _P, _P, _P, _I64] + [_P] * 7 + [_I64] * 4 + [_P, _P, _I64, _I64, _I64, _P, _INT,
+                                                                                    _INT, _P]),
+    "b200mp_pna_edge_backward": (_INT, [_P, _P, _P, _P, _I64] + [_P] * 8 + [_I64, _P] + [_I64] * 4 + [_INT, _INT, _P]),
 }
 
 _lib = None

@@ -206,6 +206,95 @@ def aggregate_gated_qv(graph: CSRGraph, k: Tensor, qv: Tensor, reduce: str = "su
     return _AggregateGated.apply(k.contiguous(), qv.contiguous(), None, graph, "mean" if reduce == "mean" else "sum")
 
 
+class _PNAAggregate(torch.autograd.Function):
+    """PNAConv's aggregation of m_e = u_i + w_e, w_e = v_j (+ c_e) (csrc/pna.cu).  The sweep collects the statistics
+    of w (b200mp_multi_aggr_csr on v, or b200mp_pna_edge_stats with c); the epilogue shifts them by u, applies the
+    scalers and writes the post-network input.  Backward: the prologue gives grad_u in closed form and the per-edge
+    terms, then one transposed-CSR sweep gives grad_v (and grad_c); each sweep runs only when its inputs need it."""
+
+    @staticmethod
+    def forward(ctx, x: Tensor, uv: Tensor, c: Optional[Tensor], avg_lin: Tensor, avg_log: Tensor, graph: CSRGraph,
+                aggrs: tuple, scalers: tuple):
+        N, T, F = x.shape
+        W = T * F
+        u, v = uv[:, :W], uv[:, W:]
+        lin32 = avg_lin.detach().reshape(1).float().contiguous()
+        log32 = avg_log.detach().reshape(1).float().contiguous()
+        need_grad = any(ctx.needs_input_grad[:5])
+        vv = None
+        if c is None:
+            vv = v.contiguous()
+            res = ops.multi_aggr_csr(graph.rowptr, graph.col, vv, graph.num_dst, ops._pna_need(aggrs), graph.plan,
+                                     with_ties=need_grad, count_self_zero=False)
+        else:
+            res = ops.pna_edge_stats(graph.rowptr, graph.col, graph.perm, v, c, graph.num_dst, aggrs, graph.plan,
+                                     with_ties=need_grad)
+        out = ops.pna_epilogue(graph.rowptr, x.reshape(N, W), u, res, aggrs, scalers, lin32, log32, T)
+        ctx.graph, ctx.aggrs, ctx.scalers, ctx.shape = graph, aggrs, scalers, (N, T, F)
+        ctx.keys, ctx.avg_dtypes = tuple(res), (avg_lin.dtype, avg_log.dtype)
+        ctx.save_for_backward(uv, vv, c, lin32, log32, *res.values())
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out: Tensor):
+        uv, vv, c, lin32, log32, *saved = ctx.saved_tensors
+        stats = dict(zip(ctx.keys, saved))
+        graph = ctx.graph
+        N, T, F = ctx.shape
+        W = T * F
+        nx, nuv, nc, nlin, nlog = ctx.needs_input_grad[:5]
+        grad_uv = torch.empty(N, 2 * W, dtype=uv.dtype, device=uv.device) if nuv else None
+        r = ops.pna_prologue(graph.rowptr, grad_out.to(uv.dtype), uv[:, :W], stats, ctx.aggrs, ctx.scalers, lin32, log32,
+                             T, want_u=nuv, want_x=nx, want_avg=nlin or nlog,
+                             grad_u=None if grad_uv is None else grad_uv[:, :W])
+        grad_c = None
+        if nuv or nc:
+            graph.build_transpose()
+            if c is None:
+                hit = stats.get("hit_mask")
+                gv = ops.multi_aggr_backward(graph.rowptr_t, graph.col_t, vv, r["term_a"], r["term_b"], stats.get("min"),
+                                             r["gmin"], stats.get("max"), r["gmax"], False, hit,
+                                             None if hit is None else graph.t2csr)
+                grad_uv[:, W:] = gv
+            else:
+                grad_c = ops.pna_edge_backward(graph.rowptr_t, graph.col_t, graph.perm_t, uv[:, W:], c, r, stats,
+                                               graph.num_dst, None if grad_uv is None else grad_uv[:, W:], nc)
+        gx = None if r["grad_x"] is None else r["grad_x"].view(N, T, F)
+        avg = r["avg"]
+        g_lin = avg[0:1].to(ctx.avg_dtypes[0]) if nlin else None
+        g_log = avg[1:2].to(ctx.avg_dtypes[1]) if nlog else None
+        return gx, grad_uv, grad_c, g_lin, g_log, None, None, None
+
+
+def pna_aggregate(graph: CSRGraph, x: Tensor, uv: Tensor, c: Optional[Tensor], aggregators, scalers,
+                  avg_deg_lin: Tensor, avg_deg_log: Tensor) -> Tensor:
+    """PNAConv's propagate + cat([x, out]) (pna_conv.py:158-188, aggr/scaler.py:75-109) for one pre-layer per tower:
+    the message of edge e = (j -> i) is u[i] + v[j] (+ c[e]) with uv = [u | v] one [N, 2W] tensor (W = towers * F)
+    and c [E, W] in the caller's edge order (None without edge features).  x: [N, towers, F] (each tower's input).
+    Returns [N, towers, (1 + A S) F] = cat([x_t, s_1(a_1 .. a_A), ..., s_S(a_1 .. a_A)]) per tower.  Gradients flow to
+    x, uv, c and the two avg_deg tensors ([1] each, as DegreeScalerAggregation holds them)."""
+    aggrs = tuple({"add": "sum"}.get(a, a) for a in aggregators)
+    scalers = tuple(scalers)
+    for a in aggrs:
+        if a not in ops.PNA_AGGRS:
+            raise ValueError(f"cannot fuse aggregator '{a}' (supported: {ops.PNA_AGGRS})")
+    for s in scalers:
+        if s not in ops.PNA_SCALERS:
+            raise ValueError(f"Unknown scaler '{s}'")
+    if len(set(aggrs)) != len(aggrs) or len(set(scalers)) != len(scalers):
+        raise ValueError("each aggregator and each scaler may appear once")
+    if x.dim() != 3:
+        raise ValueError(f"x must be [N, towers, F], got {tuple(x.shape)}")
+    N, T, F = x.shape
+    if uv.shape != (N, 2 * T * F) or uv.dtype != x.dtype:
+        raise ValueError(f"uv must be a [{N}, {2 * T * F}] tensor of x's dtype, got {tuple(uv.shape)} {uv.dtype}")
+    if N != graph.num_dst or N != graph.num_src:
+        raise ValueError(f"x has {N} rows but the graph has {graph.num_src} sources and {graph.num_dst} destinations")
+    if c is not None and (c.shape != (graph.num_edges, T * F) or c.dtype != x.dtype):
+        raise ValueError(f"c must be a [{graph.num_edges}, {T * F}] tensor of x's dtype, got {tuple(c.shape)} {c.dtype}")
+    return _PNAAggregate.apply(x.contiguous(), uv.contiguous(), c, avg_deg_lin, avg_deg_log, graph, aggrs, scalers)
+
+
 class _Segment(torch.autograd.Function):
     @staticmethod
     def forward(ctx, src: Tensor, ptr: Tensor, reduce: str):

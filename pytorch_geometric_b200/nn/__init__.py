@@ -2,4 +2,4 @@ from .aggr import (Aggregation, FusedAggregation, MaxAggregation, MeanAggregatio
                    MultiAggregation, SoftmaxAggregation, StdAggregation, SumAggregation, VarAggregation,
                    aggregation_resolver)
 from .conv import (FastRGCNConv, GATConv, GATv2Conv, GCNConv, GINConv, GINEConv, GraphConv, HeteroLinear,  # noqa: F401
-                   ResGatedGraphConv, RGCNConv, SAGEConv, TransformerConv)
+                   PNAConv, ResGatedGraphConv, RGCNConv, SAGEConv, TransformerConv)

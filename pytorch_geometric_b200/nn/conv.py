@@ -13,6 +13,7 @@ Two layers of code:
       GINConv         nn/conv/gin_conv.py:18-105         nn.*, eps [1]
       GINEConv        nn/conv/gin_conv.py:104-207        nn.*, eps [1], lin.weight/bias (edge_dim)
       ResGatedGraphConv nn/conv/res_gated_graph_conv.py:13-148  lin_key/lin_query/lin_value.weight/bias, lin_skip.weight, bias
+      PNAConv         nn/conv/pna_conv.py:20-209         aggr_module.avg_deg_lin/log, edge_encoder.*, pre_nns.t.0.*, post_nns.*, lin.*
       RGCNConv        nn/conv/rgcn_conv.py:40-300        weight [R,in,out] (or bases/blocks + comp), root, bias
       FastRGCNConv    nn/conv/rgcn_conv.py:302-374       same parameters
       GATConv         nn/conv/gat_conv.py:27-413         lin (or lin_src/lin_dst), att_src/att_dst, lin_edge/att_edge, res, bias
@@ -551,6 +552,150 @@ class ResGatedGraphConv(torch.nn.Module):
 
     def __repr__(self) -> str:
         return f"{self.__class__.__name__}({self.in_channels}, {self.out_channels})"
+
+
+def pna_uv_c(x: Tensor, edge_attr: Optional[Tensor], pre_weights, pre_biases, enc_w: Optional[Tensor],
+             enc_b: Optional[Tensor], towers: int, f_in: int, divide_input: bool):
+    """u | v ([N, 2W], W = towers * f_in) and c ([E, W] or None) from the towers' one-layer pre-transforms
+    Linear(cat(x_i, x_j[, edge_encoder(edge_attr)])) (pna_conv.py:167-188), split by weight column blocks:
+    u = x_t Wa_t^T + b_t, v = x_t Wb_t^T, c = edge_encoder(edge_attr) Wc_t^T.  Slicing and concatenating the module's
+    own parameters keeps every parameter gradient with autograd."""
+    wa = [w[:, :f_in] for w in pre_weights]
+    wb = [w[:, f_in:2 * f_in] for w in pre_weights]
+    if divide_input:                                        # tower t reads x[:, t F : (t + 1) F]: block-diagonal weights
+        w_uv = torch.cat([torch.block_diag(*wa), torch.block_diag(*wb)], dim=0)
+    else:
+        w_uv = torch.cat(wa + wb, dim=0)
+    b_uv = torch.cat(list(pre_biases) + [torch.zeros_like(b) for b in pre_biases])
+    uv = dense.linear(x, w_uv, b_uv)
+    c = None
+    if edge_attr is not None:
+        wc = torch.cat([w[:, 2 * f_in:] for w in pre_weights], dim=0)           # [W, f_in]
+        c = dense.linear(dense.linear(edge_attr, enc_w, enc_b), wc)
+    return uv, c
+
+
+def pna_block(x: Tensor, graph: CSRGraph, edge_attr: Optional[Tensor], pre_weights, pre_biases, enc_w, enc_b,
+              aggregators, scalers, avg_deg_lin: Tensor, avg_deg_log: Tensor, towers: int, f_in: int,
+              divide_input: bool) -> Tensor:
+    """PNAConv's post-network input cat([x_t, scaled aggregations]) [N, towers, (1 + A S) f_in] (pna_conv.py:158-169)."""
+    uv, c = pna_uv_c(x, edge_attr, pre_weights, pre_biases, enc_w, enc_b, towers, f_in, divide_input)
+    x3 = x.view(-1, towers, f_in) if divide_input else x.view(-1, 1, f_in).expand(-1, towers, f_in)
+    return Fn.pna_aggregate(graph, x3, uv, c, aggregators, scalers, avg_deg_lin, avg_deg_log)
+
+
+_ACTS = {"relu": torch.nn.ReLU, "elu": torch.nn.ELU, "leaky_relu": torch.nn.LeakyReLU, "gelu": torch.nn.GELU,
+         "tanh": torch.nn.Tanh, "sigmoid": torch.nn.Sigmoid, "silu": torch.nn.SiLU, "swish": torch.nn.SiLU}
+
+
+def _activation(act, act_kwargs):
+    if isinstance(act, str):
+        key = act.lower().replace("_", "")
+        for name, cls in _ACTS.items():
+            if name.replace("_", "") == key:
+                return cls(**(act_kwargs or {}))
+        raise ValueError(f"Could not resolve '{act}' among choices {sorted(_ACTS)}")
+    if isinstance(act, type):
+        return act(**(act_kwargs or {}))
+    return act
+
+
+class _DegreeScalerState(torch.nn.Module):
+    """avg_deg_lin / avg_deg_log of DegreeScalerAggregation (nn/aggr/scaler.py:60-75): buffers, or parameters with
+    train_norm, initialised from the in-degree histogram."""
+
+    def __init__(self, deg: Tensor, train_norm: bool):
+        super().__init__()
+        deg = deg.to(torch.float)
+        n = float(deg.sum())
+        bins = torch.arange(deg.numel(), device=deg.device, dtype=torch.float)
+        self.init_avg_deg_lin = float((bins * deg).sum()) / n
+        self.init_avg_deg_log = float(((bins + 1).log() * deg).sum()) / n
+        if train_norm:
+            self.avg_deg_lin = torch.nn.Parameter(torch.empty(1))
+            self.avg_deg_log = torch.nn.Parameter(torch.empty(1))
+        else:
+            self.register_buffer("avg_deg_lin", torch.empty(1))
+            self.register_buffer("avg_deg_log", torch.empty(1))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        self.avg_deg_lin.data.fill_(self.init_avg_deg_lin)
+        self.avg_deg_log.data.fill_(self.init_avg_deg_log)
+
+
+class PNAConv(torch.nn.Module):
+    """Principal Neighbourhood Aggregation (pna_conv.py:20-209) with one pre-layer per tower: the towers' message
+    Linear is split into per-node products and the per-edge c (with `edge_dim`), and the aggregators in {sum, mean,
+    min, max, var, std} with the five degree scalers run as one CSR sweep plus node-level kernels
+    (`Fn.pna_aggregate`).  `pre_layers != 1` and other aggregators or scalers raise ValueError."""
+
+    def __init__(self, in_channels: int, out_channels: int, aggregators, scalers, deg: Tensor,
+                 edge_dim: Optional[int] = None, towers: int = 1, pre_layers: int = 1, post_layers: int = 1,
+                 divide_input: bool = False, act="relu", act_kwargs=None, train_norm: bool = False, **kwargs):
+        super().__init__()
+        if pre_layers != 1:
+            raise ValueError(f"pre_layers={pre_layers} is not on the fused path (only one pre-layer per tower is)")
+        aggregators = [aggregators] if isinstance(aggregators, str) else list(aggregators)
+        scalers = [scalers] if isinstance(scalers, str) else list(scalers)
+        for a in aggregators:
+            if {"add": "sum"}.get(a, a) not in ops.PNA_AGGRS:
+                raise ValueError(f"aggregator '{a}' is not on the fused path (supported: {ops.PNA_AGGRS})")
+        for sc in scalers:
+            if sc not in ops.PNA_SCALERS:
+                raise ValueError(f"Unknown scaler '{sc}'")
+        if divide_input:
+            assert in_channels % towers == 0
+        assert out_channels % towers == 0
+        self.aggregators, self.scalers = aggregators, scalers
+        self.flow = kwargs.get("flow", "source_to_target")
+        self.in_channels, self.out_channels, self.edge_dim = in_channels, out_channels, edge_dim
+        self.towers, self.divide_input = towers, divide_input
+        self.F_in = in_channels // towers if divide_input else in_channels
+        self.F_out = out_channels // towers
+        self.aggr_module = _DegreeScalerState(deg, train_norm)
+        if edge_dim is not None:
+            self.edge_encoder = _Lin(edge_dim, self.F_in)
+        self.pre_nns = torch.nn.ModuleList(
+            [torch.nn.Sequential(_Lin((3 if edge_dim else 2) * self.F_in, self.F_in)) for _ in range(towers)])
+        self.post_nns = torch.nn.ModuleList()
+        for _ in range(towers):
+            mods = [_Lin((len(aggregators) * len(scalers) + 1) * self.F_in, self.F_out)]
+            for _ in range(post_layers - 1):
+                mods += [_activation(act, act_kwargs), _Lin(self.F_out, self.F_out)]
+            self.post_nns.append(torch.nn.Sequential(*mods))
+        self.lin = _Lin(out_channels, out_channels)
+
+    def forward(self, x: Tensor, edge_index: Adj, edge_attr: Optional[Tensor] = None) -> Tensor:
+        graph = _plain_graph(edge_index, x.size(0), x.size(0), self.flow)
+        enc = getattr(self, "edge_encoder", None)
+        block = pna_block(x, graph, edge_attr if self.edge_dim is not None else None,
+                          [nn[0].weight for nn in self.pre_nns], [nn[0].bias for nn in self.pre_nns],
+                          _w(enc), None if enc is None else enc.bias, self.aggregators, self.scalers,
+                          self.aggr_module.avg_deg_lin, self.aggr_module.avg_deg_log, self.towers, self.F_in,
+                          self.divide_input)
+        # unbind: one [N, T, (1 + A S) F] gradient for all towers, where block[:, t] would allocate one per tower
+        out = torch.cat([nn(b) for nn, b in zip(self.post_nns, block.unbind(1))], dim=1)
+        return self.lin(out)
+
+    def __repr__(self) -> str:
+        return (f"{self.__class__.__name__}({self.in_channels}, {self.out_channels}, towers={self.towers}, "
+                f"edge_dim={self.edge_dim})")
+
+    @staticmethod
+    def get_degree_histogram(loader) -> Tensor:
+        """Histogram of the in-degrees of every graph in `loader` (index = degree), for the `deg` argument."""
+        hist = torch.zeros(1, dtype=torch.long)
+        for data in loader:
+            dst = data.edge_index[1]
+            deg = torch.zeros(data.num_nodes, dtype=torch.long, device=dst.device).index_add_(
+                0, dst, torch.ones_like(dst, dtype=torch.long))
+            counts = torch.bincount(deg, minlength=hist.numel())
+            hist = hist.to(counts.device)
+            if counts.numel() > hist.numel():
+                hist = torch.cat([hist, hist.new_zeros(counts.numel() - hist.numel())])
+            hist = hist + counts
+        return hist
 
 
 class RGCNConv(torch.nn.Module):

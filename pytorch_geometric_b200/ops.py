@@ -6,6 +6,7 @@ no CPU fallback.
 """
 from __future__ import annotations
 
+import ctypes
 from typing import Optional, Tuple
 
 import torch
@@ -906,6 +907,133 @@ def multi_aggr_backward(ptr: Optional[Tensor], idx: Tensor, x: Tensor, term_a: O
            _p(term_b), _p(out_min), _p(g_min), _p(out_max), _p(g_max), _p(hit_mask), _p(t2csr), _p(gx), x.size(0), x.size(1),
            int(bool(segment_mode)), it, _vdt(x), _stream())
     return gx
+
+
+PNA_AGGRS = ("sum", "mean", "min", "max", "var", "std")
+PNA_SCALERS = ("identity", "amplification", "attenuation", "linear", "inverse_linear")
+
+
+def _host_codes(names, table):
+    """int32 host array of the codes of `names` in `table` (the C ABI reads it during the call)."""
+    return (ctypes.c_int32 * len(names))(*[table.index(n) for n in names])
+
+
+def _pna_stats_args(stats: dict):
+    return [_p(stats.get(k)) for k in ("sum", "min", "max", "var")]
+
+
+def _pna_stats_dtype(stats: dict, ref: Tensor) -> int:
+    ts = [t for k, t in stats.items() if k in ("sum", "min", "max", "var") and t is not None]
+    return _vdt(ts[0]) if ts else _vdt(ref)
+
+
+def pna_epilogue(rowptr: Tensor, x: Tensor, u: Tensor, stats: dict, aggrs, scalers, avg_deg_lin: Tensor,
+                 avg_deg_log: Tensor, towers: int) -> Tensor:
+    """[N, towers, (1 + A S) F] = cat([x_t, scaler_1(aggr_1 .. aggr_A), ...]) per tower from the statistics of w
+    (`stats`: 'sum' / 'min' / 'max' / 'var' planes [N, W]) shifted by u ([N, W], row stride u.stride(0)); x: [N, W]."""
+    _cuda(rowptr, x, u, avg_deg_lin, avg_deg_log, *stats.values())
+    N, W = x.shape
+    F = W // towers
+    if u.stride(1) != 1:
+        u = u.contiguous()
+    out = torch.empty(N, towers, (1 + len(aggrs) * len(scalers)) * F, dtype=x.dtype, device=x.device)
+    ac, sc = _host_codes(aggrs, PNA_AGGRS), _host_codes(scalers, PNA_SCALERS)
+    _timed("pna_epilogue", 1, lib().b200mp_pna_epilogue, _p(rowptr), _p(x.contiguous()), _p(u), u.stride(0),
+           *_pna_stats_args(stats), ctypes.addressof(ac), len(aggrs), ctypes.addressof(sc),
+           len(scalers), _p(avg_deg_lin), _p(avg_deg_log), _p(out), N, towers, F, _pna_stats_dtype(stats, x),
+           _idt(rowptr), _vdt(x), _stream())
+    return out
+
+
+def pna_prologue(rowptr: Tensor, grad_out: Tensor, u: Tensor, stats: dict, aggrs, scalers, avg_deg_lin: Tensor,
+                 avg_deg_log: Tensor, towers: int, want_u: bool, want_x: bool, want_avg: bool, grad_u: Optional[Tensor] = None):
+    """Backward prologue of pna_epilogue: dict with the fp32 [N, W] rows the sweep backward reads ('term_a', 'term_b',
+    'gmin', 'gmax', each present only when an aggregator needs it), 'grad_u' (written into `grad_u` when given, e.g.
+    the left half of an [N, 2W] gradient), 'grad_x' [N, W] and 'avg' = (d L / d avg_deg_lin, d L / d avg_deg_log)."""
+    _cuda(rowptr, grad_out, u, avg_deg_lin, avg_deg_log, *stats.values())
+    grad_out = grad_out.contiguous()
+    N = grad_out.size(0)
+    W = u.size(1)
+    F = W // towers
+    dev = grad_out.device
+    new = lambda: torch.empty(N, W, dtype=torch.float32, device=dev)       # noqa: E731
+    res = {
+        "term_a": new() if any(a in aggrs for a in ("sum", "mean", "var", "std")) else None,
+        "term_b": new() if any(a in aggrs for a in ("var", "std")) else None,
+        "gmin": new() if "min" in aggrs else None,
+        "gmax": new() if "max" in aggrs else None,
+    }
+    if want_u and grad_u is None:
+        grad_u = torch.empty(N, W, dtype=grad_out.dtype, device=dev)
+    res["grad_u"] = grad_u if want_u else None
+    res["grad_x"] = torch.empty(N, W, dtype=grad_out.dtype, device=dev) if want_x else None
+    part = torch.empty(N, 2, dtype=torch.float32, device=dev) if want_avg else None
+    if u.stride(1) != 1:
+        u = u.contiguous()
+    gu = res["grad_u"]
+    ac, sc = _host_codes(aggrs, PNA_AGGRS), _host_codes(scalers, PNA_SCALERS)
+    _timed("pna_prologue", 1, lib().b200mp_pna_prologue, _p(rowptr), _p(grad_out), _p(u), u.stride(0),
+           *_pna_stats_args(stats), _p(stats.get("ties_min")), _p(stats.get("ties_max")),
+           ctypes.addressof(ac), len(aggrs), ctypes.addressof(sc), len(scalers),
+           _p(avg_deg_lin), _p(avg_deg_log), _p(res["term_a"]), _p(res["term_b"]), _p(res["gmin"]), _p(res["gmax"]),
+           _p(gu), gu.stride(0) if gu is not None else W, _p(res["grad_x"]), _p(part), N, towers, F,
+           _pna_stats_dtype(stats, grad_out), _idt(rowptr), _vdt(grad_out), _stream())
+    res["avg"] = None if part is None else column_sum(part)
+    return res
+
+
+def pna_edge_stats(rowptr: Tensor, col: Tensor, perm: Optional[Tensor], v: Tensor, c: Tensor, n_rows: int, aggrs,
+                   plan: Optional[LongRowPlan] = None, with_ties: bool = False) -> dict:
+    """fp32 statistics of w_e = v[col[e]] + c[perm[e]] per destination row ('sum', 'min', 'max', 'var', and with_ties
+    'ties_min' / 'ties_max'), only those the aggregators need.  v: [n_cols, W] (row stride v.stride(0)); c: [E, W]
+    in the caller's edge order."""
+    _cuda(rowptr, col, perm, v, c)
+    W = v.size(1)
+    if v.stride(1) != 1:
+        v = v.contiguous()
+    c = c.contiguous()
+    need = _pna_need(aggrs)
+    st = {k: torch.empty(n_rows, W, dtype=torch.float32, device=v.device) for k in need}
+    if with_ties:
+        for k in ("min", "max"):
+            if k in st:
+                st["ties_" + k] = torch.empty(n_rows, W, dtype=torch.float32, device=v.device)
+    pargs, _ = _plan_args(plan, 6 * W, v.device)
+    _timed("pna_edge_stats", 2 if pargs[2] else 1, lib().b200mp_pna_edge_stats, _p(rowptr), _p(col), _p(perm), _p(v),
+           v.stride(0), _p(c), _p(st.get("sum")), _p(st.get("min")), _p(st.get("max")), _p(st.get("var")),
+           _p(st.get("ties_min")), _p(st.get("ties_max")), n_rows, v.size(0), col.numel(), W, *pargs,
+           _same_idx(rowptr, col, perm), _vdt(v), _stream())
+    return st
+
+
+def _pna_need(aggrs) -> tuple:
+    """The statistics of w an aggregator list reads."""
+    need = []
+    if any(a in aggrs for a in ("sum", "mean", "var", "std")):
+        need.append("sum")
+    need += [a for a in ("min", "max") if a in aggrs]
+    if any(a in aggrs for a in ("var", "std")):
+        need.append("var")
+    return tuple(need)
+
+
+def pna_edge_backward(rowptr_t: Tensor, col_t: Tensor, perm_t: Tensor, v: Tensor, c: Tensor, terms: dict, stats: dict,
+                      n_dst: int, grad_v: Optional[Tensor], want_c: bool) -> Optional[Tensor]:
+    """One transposed-CSR sweep: d L / d w_e into grad_c [E, W] (caller's order, returned when want_c) and its sum over
+    every source's out-edges into grad_v (written in place, row stride grad_v.stride(0); may be None)."""
+    _cuda(rowptr_t, col_t, perm_t, v, c, grad_v)
+    W = v.size(1)
+    if v.stride(1) != 1:
+        v = v.contiguous()
+    c = c.contiguous()
+    E = c.size(0)
+    grad_c = torch.empty(E, W, dtype=c.dtype, device=c.device) if want_c else None
+    _timed("pna_edge_backward", 1, lib().b200mp_pna_edge_backward, _p(rowptr_t), _p(col_t), _p(perm_t), _p(v),
+           v.stride(0), _p(c), _p(terms.get("term_a")), _p(terms.get("term_b")), _p(stats.get("min")),
+           _p(terms.get("gmin")), _p(stats.get("max")), _p(terms.get("gmax")), _p(grad_v),
+           grad_v.stride(0) if grad_v is not None else W, _p(grad_c), v.size(0), n_dst, E, W,
+           _same_idx(rowptr_t, col_t, perm_t), _vdt(v), _stream())
+    return grad_c
 
 
 def device_info() -> dict:

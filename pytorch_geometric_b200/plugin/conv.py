@@ -35,7 +35,7 @@ from ._util import plain
 # Inspector caches class sources by `cls.__name__` (torch_geometric/inspector.py:323-334), so a subclass that reused
 # its parent's name would hide the parent's `# propagate_type:` annotation and get a `propagate` without arguments.
 LAYERS = {n: "B200" + n for n in ("GCNConv", "SAGEConv", "GraphConv", "GINConv", "GATConv", "GATv2Conv", "TransformerConv",
-                                  "RGCNConv", "FastRGCNConv")}
+                                  "RGCNConv", "FastRGCNConv", "PNAConv")}
 
 
 def _has_hooks(self) -> bool:
@@ -271,3 +271,50 @@ class B200RGCNConv(_RGCNMixin, tgnn.RGCNConv):
 
 class B200FastRGCNConv(_RGCNMixin, tgnn.FastRGCNConv):
     pass
+
+
+def _pna_fusable(self, x, edge_index, edge_attr) -> bool:
+    """The fused PNA path covers one Linear per pre-network, aggregators in {sum, mean, min, max, var, std} once each,
+    the five scalers once each, a [2, E] / EdgeIndex adjacency and CUDA float32 / bfloat16 inputs."""
+    if not (isinstance(x, Tensor) and x.dim() == 2 and _fast(self, x, edge_attr)):
+        return False
+    if not (isinstance(edge_index, Tensor) and edge_index.layout == torch.strided and edge_index.dim() == 2
+            and edge_index.size(0) == 2 and not edge_index.is_floating_point()):
+        return False
+    if any(len(nn) != 1 or not isinstance(nn[0], tgnn.Linear) for nn in self.pre_nns):
+        return False
+    if (edge_attr is None) != (self.edge_dim is None) or (edge_attr is not None and edge_attr.dim() != 2):
+        return False
+    aggr = self.aggr_module
+    if not isinstance(aggr, tgnn.aggr.DegreeScalerAggregation):
+        return False
+    inner = aggr.aggr.aggrs if isinstance(aggr.aggr, tgnn.aggr.MultiAggregation) else [aggr.aggr]
+    names = [_PNA_AGGRS.get(type(a)) for a in inner]
+    if None in names or len(set(names)) != len(names) or any(getattr(a, "semi_grad", False) for a in inner):
+        return False
+    if any(getattr(a, "var_aggr", None) is not None and a.var_aggr.semi_grad for a in inner):
+        return False
+    sc = list(aggr.scaler)
+    return all(s in ("identity", "amplification", "attenuation", "linear", "inverse_linear") for s in sc) and len(set(sc)) == len(sc)
+
+
+_PNA_AGGRS = {tgnn.aggr.SumAggregation: "sum", tgnn.aggr.MeanAggregation: "mean", tgnn.aggr.MinAggregation: "min",
+              tgnn.aggr.MaxAggregation: "max", tgnn.aggr.VarAggregation: "var", tgnn.aggr.StdAggregation: "std"}
+
+
+class B200PNAConv(tgnn.PNAConv):
+    def forward(self, x, edge_index, edge_attr=None) -> Tensor:
+        if _pna_fusable(self, x, edge_index, edge_attr):
+            g = _graph(edge_index, x.size(0), x.size(0), self.flow)
+            if g is not None:
+                aggr = self.aggr_module
+                inner = aggr.aggr.aggrs if isinstance(aggr.aggr, tgnn.aggr.MultiAggregation) else [aggr.aggr]
+                enc = getattr(self, "edge_encoder", None)
+                block = C.pna_block(x, g, edge_attr, [nn[0].weight for nn in self.pre_nns], [nn[0].bias for nn in self.pre_nns],
+                                    None if enc is None else enc.weight, None if enc is None else enc.bias,
+                                    [_PNA_AGGRS[type(a)] for a in inner], list(aggr.scaler), aggr.avg_deg_lin,
+                                    aggr.avg_deg_log, self.towers, self.F_in, self.divide_input)
+                # unbind: one [N, T, (1 + A S) F] gradient for all towers, where block[:, t] would allocate one per tower
+                out = torch.cat([nn(b) for nn, b in zip(self.post_nns, block.unbind(1))], dim=1)   # pna_conv.py:170-173
+                return self.lin(out)
+        return super().forward(x, edge_index, edge_attr)

@@ -18,7 +18,7 @@ int csr_reduce_variant(const I* rowptr, const I* col, const float* val, const T*
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     const size_t row_bytes = static_cast<size_t>(feat) * sizeof(T);
     const bool tma_ok = row_bytes % 16 == 0 && row_bytes >= 512 && row_bytes <= 2048 && aligned16(x) &&
-                        aligned16(out) && (plan.n_chunks == 0 || aligned16(plan.partials));
+                        aligned16(plan.x2) && aligned16(out) && (plan.n_chunks == 0 || aligned16(plan.partials));
     // "auto" is the lane-group kernel: at 48 warps/SM it keeps more rows in flight than the TMA-fed
     // kernel, which is issue-bound at 6 warps/SM.  The TMA variant stays selectable for A/B timing.
     const int impl = get_option_spmm_impl();

@@ -360,8 +360,9 @@ int csr_reduce_dispatch(const I* rowptr, const I* col, const float* val, const T
                         LongRowPlan plan, const float* bias, cudaStream_t stream) {
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     const size_t row_bytes = static_cast<size_t>(feat) * sizeof(T);
-    const bool vec_ok = (row_bytes % 16 == 0) && aligned16(x) && aligned16(out) &&
-                        (plan.n_chunks == 0 || aligned16(plan.partials));
+    // every matrix the vector kernel reads or writes with 128-bit accesses: the halo segment and the ReLU mask too
+    const bool vec_ok = (row_bytes % 16 == 0) && aligned16(x) && aligned16(out) && aligned16(plan.x2) &&
+                        aligned16(plan.relu_mask) && (plan.n_chunks == 0 || aligned16(plan.partials));
     if (vec_ok) {
         const int n_vec = static_cast<int>(row_bytes / 16);
 #define B200MP_LV(G_, V_) \

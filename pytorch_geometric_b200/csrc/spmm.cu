@@ -144,6 +144,9 @@ extern "C" int b200mp_spmm_csr(const void* rowptr, const void* col, const float*
     B200MP_CHECK_ARG(rowptr && out);
     B200MP_CHECK_ARG(x || n_cols == 0 || peer_ptrs);
     B200MP_CHECK_ARG(!peer_ptrs || (peer_rows > 0 && !x_halo && (feat * (val_dtype == B200MP_BF16 ? 2 : 4)) % 16 == 0));
+    // the scalar fallback, taken when a matrix is not 16-byte aligned, has no peer-table addressing
+    B200MP_CHECK_ARG(!peer_ptrs || (aligned16(x) && aligned16(out) && aligned16(relu_mask) &&
+                                    (n_long_rows == 0 || aligned16(partials))));
     B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);
     B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && partials && chunk > 0));
     B200MP_CHECK_ARG(!x_halo || (n_local_cols >= 0 && n_local_cols <= n_cols));

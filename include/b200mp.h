@@ -264,6 +264,52 @@ int b200mp_gated_backward_src(const void* rowptr_t, const void* col_t, const flo
                               int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials,
                               int idx_dtype, int val_dtype, void* stream);
 
+/* ------------------------------------------------------------------ crystal-graph message sigmoid(f) * softplus(s)
+ * out[i, :] = REDUCE_{e in [rowptr[i], rowptr[i+1])} sigmoid(f_e) * softplus(s_e),  REDUCE = sum | mean, with
+ * f_e = u[i, 0:F] + v[col[e], 0:F] (+ c[eid(e), 0:F]) and s_e = u[i, F:2F] + v[col[e], F:2F] (+ c[eid(e), F:2F]).
+ * Replaces: CGConv.message + aggregate (nn/conv/cg_conv.py:93-98 with message_passing.py:263-333 and
+ * aggr/base.py:173-185): the reference materialises x_i, x_j, their concatenation with edge_attr, both Linear outputs,
+ * the sigmoid, the softplus and the product, all [E, *] tensors.  u and v are the per-node column blocks of both
+ * Linears (u carries the biases), c the edge_attr block.
+ * u: [n_rows, 2F] rows with row stride ld_u >= 2F; v: [n_cols, 2F] rows with stride ld_v >= 2F (u and v may be the
+ * two halves of one [N, 4F] product); c: [n_edges, 2F] contiguous in the CALLER's edge order, or NULL; eid(e) =
+ * perm[e], or e when perm is NULL (an adopted CSR); out: [n_rows, F]; all val_dtype.  f and s are summed in fp32 and
+ * rounded to val_dtype once (the reference's Linear output); sigmoid, softplus (ATen threshold 20) and their product
+ * are each rounded to val_dtype; fp32 accumulation in CSR order; mean divides by max(deg, 1); empty rows give 0.
+ * Long rows: plan and partials ([n_chunks, F] fp32) as in b200mp_spmm_csr. */
+int b200mp_cg_csr(const void* rowptr, const void* col, const void* perm, const void* u, const void* v,
+                  const void* c, void* out, int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t feat,
+                  int64_t ld_u, int64_t ld_v, int reduce, const int64_t* long_rows,
+                  const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks, int64_t chunk,
+                  float* partials, int idx_dtype, int val_dtype, void* stream);
+/* grad_u (and grad_c) of b200mp_cg_csr over the destination CSR (replaces the autograd of cg_conv.py:98 wrt x_i and
+ * edge_attr: mul, sigmoid, softplus and Linear backward over E rows, then the index_select backward through
+ * index_add_ atomics).  With g_i = grad_out[i, :] / (mean ? max(deg_i, 1) : 1):
+ *   df_e = g_i * sigmoid'(f_e) * softplus(s_e),  ds_e = g_i * sigmoid(f_e) * softplus'(s_e)
+ *   grad_u[i, :] = sum_{e in row i} [df_e | ds_e]   ([n_rows, 2F] rows with stride ld_u; 0 for a row without edges)
+ *   grad_c[eid(e), :] = [df_e | ds_e]               ([n_edges, 2F], caller's edge order; NULL: not written;
+ *                                                    given only with c)
+ * Long rows: plan and partials ([n_chunks, 2F] fp32). */
+int b200mp_cg_backward_dst(const void* rowptr, const void* col, const void* perm, const void* u,
+                           const void* v, const void* c, const void* grad_out, void* grad_u, void* grad_c,
+                           int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t feat, int64_t ld_u,
+                           int64_t ld_v, int reduce, const int64_t* long_rows, const int64_t* chunk_ptr,
+                           int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials,
+                           int idx_dtype, int val_dtype, void* stream);
+/* grad_v of b200mp_cg_csr by ONE sweep over the TRANSPOSED CSR (replaces the index_select backward wrt x_j):
+ *   grad_v[j, :] = sum_{t in rowT(j)} [df_t | ds_t] with g = w_t * grad_out[col_t[t], :]
+ * w_t = val_t[t] (nullable, fp32: 1 / max(deg, 1) of the destination for mean) or 1; c is read at perm_t[t], the
+ * caller's edge id of transposed slot t.  grad_v: [n_src, 2F] rows with stride ld_v; 0 for a source without
+ * out-edges.  When grad_c was written, the segment sum of its rows (b200mp_spmm_csr over rowptr_t with perm_t as the
+ * column) gives the same grad_v with fewer bytes.  Long source rows: the transposed CSR's plan, partials
+ * [n_chunks, 2F] fp32. */
+int b200mp_cg_backward_src(const void* rowptr_t, const void* col_t, const void* perm_t, const float* val_t,
+                           const void* u, const void* v, const void* c, const void* grad_out, void* grad_v,
+                           int64_t n_src, int64_t n_dst, int64_t n_edges, int64_t feat, int64_t ld_u,
+                           int64_t ld_v, const int64_t* long_rows, const int64_t* chunk_ptr,
+                           int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials,
+                           int idx_dtype, int val_dtype, void* stream);
+
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)
  * out[index[e], :] (+)= src[e, :] for an UNSORTED index.  Replaces utils/_scatter.py:14-138
  * (aten::scatter_add_ / scatter_reduce_, torch_scatter.scatter).  fp32 only.  `count` is a

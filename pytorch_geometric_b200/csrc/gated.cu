@@ -23,6 +23,7 @@
 // row-wise factor g_i or v[j] is applied after the fold).  Rows that are not a whole number of aligned 16-byte vectors
 // take a one-warp scalar kernel.
 #include "csr_reduce.cuh"
+#include "gate_math.cuh"
 
 namespace b200mp {
 
@@ -40,20 +41,6 @@ struct GatedArgs {
     int64_t ld;
     bool is_mean;
 };
-
-template <typename T>
-__device__ __forceinline__ float round_to(float v) {
-    return ElemTraits<T>::to_float(ElemTraits<T>::from_float(v));
-}
-
-// sigma(s) and sigma'(s) from t = exp(-|s|) (see the header).
-__device__ __forceinline__ void sigmoid_pair(float s, float& sig, float& dsig) {
-    const float t = __expf(-fabsf(s));
-    const float r = __fdividef(1.0f, 1.0f + t);
-    const float tr = __fmul_rn(t, r);
-    sig = s >= 0.0f ? r : tr;
-    dsig = __fmul_rn(tr, r);
-}
 
 // One (edge, feature) term.  fwd / dst: a = q[j], b = v[j], rowop = k[i]; src: a = k[i], b = g[i] (times w), rowop = q[j].
 template <typename T, int MODE>

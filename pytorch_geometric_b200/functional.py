@@ -206,6 +206,96 @@ def aggregate_gated_qv(graph: CSRGraph, k: Tensor, qv: Tensor, reduce: str = "su
     return _AggregateGated.apply(k.contiguous(), qv.contiguous(), None, graph, "mean" if reduce == "mean" else "sum")
 
 
+class _AggregateCG(torch.autograd.Function):
+    """sigmoid(f) * softplus(s) reduced by sum / mean, [f | s] = u_i + v_j (+ c_e) (csrc/cg.cu).  Nothing per edge is
+    saved: the backward recomputes f and s.  The destination sweep gives grad_u and, when c needs a gradient, grad_c;
+    grad_v is then the segment sum of grad_c's rows over the transposed CSR, and otherwise one transposed sweep.  Each
+    sweep runs only when one of its outputs is needed.  `v` None means `u` is one [N, 4F] tensor holding u | v."""
+
+    @staticmethod
+    def forward(ctx, u: Tensor, v: Optional[Tensor], c: Optional[Tensor], graph: CSRGraph, reduce: str):
+        W = u.size(1) // (2 if v is None else 1)
+        uu, vv = (u, v) if v is not None else (u[:, :W], u[:, W:])
+        out = ops.cg_csr(graph.rowptr, graph.col, graph.perm, uu, vv, c, graph.num_dst, reduce, graph.plan)
+        ctx.graph, ctx.reduce, ctx.packed = graph, reduce, v is None
+        ctx.save_for_backward(u, v, c)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out: Tensor):
+        u, v, c = ctx.saved_tensors
+        graph, reduce, packed = ctx.graph, ctx.reduce, ctx.packed
+        W = u.size(1) // (2 if packed else 1)
+        uu, vv = (u[:, :W], u[:, W:]) if packed else (u, v)
+        need_u, need_c = ctx.needs_input_grad[0], ctx.needs_input_grad[2]
+        need_v = need_u if packed else ctx.needs_input_grad[1]
+        grad_out = grad_out.contiguous()
+        gu = gv = gc = None
+        gu_dst = gv_dst = None                         # where the sweeps write: u's and v's shape and row stride
+        if packed:
+            if need_u or need_c:
+                full = torch.empty_like(u)
+                gu_dst, gv_dst = full[:, :W], full[:, W:]
+                gu = full if need_u else None
+        else:
+            if need_u or need_c:
+                gu_dst = torch.empty_like(u)
+                gu = gu_dst if need_u else None
+        if need_u or need_c:
+            gc = ops.cg_backward_dst(graph.rowptr, graph.col, graph.perm, uu, vv, c, grad_out, gu_dst, need_c, reduce,
+                                     graph.plan)
+        if need_v:
+            graph.build_transpose()
+            if gc is not None:
+                # grad_v[j] = the sum of grad_c over j's out-edges: perm_t is the caller's edge id of each transposed slot
+                sums = ops.spmm_csr(graph.rowptr_t, graph.perm_t, None, gc, graph.num_src, "sum", graph.plan_t)
+                if packed:
+                    gv_dst.copy_(sums)
+                else:
+                    gv = sums
+            else:
+                if not packed:
+                    gv = gv_dst = torch.empty_like(v)
+                val_t = graph.mean_val_t() if reduce == "mean" else None
+                ops.cg_backward_src(graph.rowptr_t, graph.col_t, graph.perm_t, val_t, uu, vv, c, grad_out, gv_dst,
+                                    graph.plan_t)
+        return gu, gv, gc, None, None
+
+
+def _cg_check(graph: CSRGraph, u: Tensor, c: Optional[Tensor], reduce: str, width: int, name: str) -> None:
+    if reduce not in ("sum", "add", "mean"):
+        raise ValueError(f"{name} reduces by sum or mean, got '{reduce}'")
+    if u.dim() != 2 or u.size(1) % width:
+        raise ValueError(f"{name}: u must be a [num_dst, {width}F] tensor, got {tuple(u.shape)}")
+    if u.size(0) != graph.num_dst:
+        raise ValueError(f"u has {u.size(0)} rows but the graph has {graph.num_dst} destination nodes")
+    F = u.size(1) // width
+    if c is not None and (tuple(c.shape) != (graph.num_edges, 2 * F) or c.dtype != u.dtype):
+        raise ValueError(f"c must be a [{graph.num_edges}, {2 * F}] tensor of u's dtype, got {tuple(c.shape)} {c.dtype}")
+
+
+def aggregate_cg(graph: CSRGraph, u: Tensor, v: Tensor, c: Optional[Tensor] = None, reduce: str = "sum") -> Tensor:
+    """out[i] = REDUCE_{e = (j -> i)} sigmoid(f_e) * softplus(s_e) for reduce in {sum, mean}, with [f_e | s_e] =
+    u[i] + v[j] (+ c[e]): CGConv's message and aggregation (cg_conv.py:93-98) with its two Linears split by weight
+    column blocks (`nn.conv.cg_uvc`).  u: [num_dst, 2F] (f half, then s half); v: [num_src, 2F]; c: [E, 2F] in the
+    caller's edge order or None; one dtype; all three may require grad.  Returns [num_dst, F]; empty rows give 0."""
+    _cg_check(graph, u, c, reduce, 2, "aggregate_cg")
+    if v.dtype != u.dtype or v.shape != (graph.num_src, u.size(1)):
+        raise ValueError(f"v must be a [{graph.num_src}, {u.size(1)}] tensor of u's dtype, got {tuple(v.shape)} {v.dtype}")
+    return _AggregateCG.apply(u.contiguous(), v.contiguous(), None if c is None else c.contiguous(), graph,
+                              "mean" if reduce == "mean" else "sum")
+
+
+def aggregate_cg_uv(graph: CSRGraph, uv: Tensor, c: Optional[Tensor] = None, reduce: str = "sum") -> Tensor:
+    """aggregate_cg with u and v as the two halves of one [N, 4F] tensor (one product of a non-bipartite layer), read
+    in place; its gradient is one [N, 4F] tensor as well.  The graph must have N sources and N destinations."""
+    _cg_check(graph, uv, c, reduce, 4, "aggregate_cg_uv")
+    if graph.num_src != graph.num_dst:
+        raise ValueError(f"aggregate_cg_uv needs as many sources as destinations, got {graph.num_src} and {graph.num_dst}")
+    return _AggregateCG.apply(uv.contiguous(), None, None if c is None else c.contiguous(), graph,
+                              "mean" if reduce == "mean" else "sum")
+
+
 class _PNAAggregate(torch.autograd.Function):
     """PNAConv's aggregation of m_e = u_i + w_e, w_e = v_j (+ c_e) (csrc/pna.cu).  The sweep collects the statistics
     of w (b200mp_multi_aggr_csr on v, or b200mp_pna_edge_stats with c); the epilogue shifts them by u, applies the

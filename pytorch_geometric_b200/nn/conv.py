@@ -13,6 +13,7 @@ Two layers of code:
       GINConv         nn/conv/gin_conv.py:18-105         nn.*, eps [1]
       GINEConv        nn/conv/gin_conv.py:104-207        nn.*, eps [1], lin.weight/bias (edge_dim)
       ResGatedGraphConv nn/conv/res_gated_graph_conv.py:13-148  lin_key/lin_query/lin_value.weight/bias, lin_skip.weight, bias
+      CGConv          nn/conv/cg_conv.py:12-101          lin_f.weight/bias, lin_s.weight/bias, bn.* (batch_norm)
       PNAConv         nn/conv/pna_conv.py:20-209         aggr_module.avg_deg_lin/log, edge_encoder.*, pre_nns.t.0.*, post_nns.*, lin.*
       RGCNConv        nn/conv/rgcn_conv.py:40-300        weight [R,in,out] (or bases/blocks + comp), root, bias
       FastRGCNConv    nn/conv/rgcn_conv.py:302-374       same parameters
@@ -552,6 +553,59 @@ class ResGatedGraphConv(torch.nn.Module):
 
     def __repr__(self) -> str:
         return f"{self.__class__.__name__}({self.in_channels}, {self.out_channels})"
+
+
+def cg_uvc(x, edge_attr: Optional[Tensor], w_f: Tensor, b_f: Optional[Tensor], w_s: Tensor, b_s: Optional[Tensor]):
+    """(u, v, c) of CGConv's message (cg_conv.py:93-98) with lin_f and lin_s split by the column blocks of
+    z = [x_i, x_j, edge_attr]: u = x_dst [W_f,a; W_s,a]^T + [b_f; b_s], v = x_src [W_f,b; W_s,b]^T and
+    c = edge_attr [W_f,c; W_s,c]^T ([E, 2F], None without edge_attr).  For one node tensor x, u | v come from one
+    [N, 4F] product and are returned as (uv, None, c); for a pair (x_src, x_dst), one product per side.  Slicing and
+    concatenating the module's own parameters keeps every parameter gradient with autograd."""
+    x_src, x_dst = (x, x) if isinstance(x, Tensor) else (x[0], x[1])
+    fd, fs = x_dst.size(-1), x_src.size(-1)
+    w = torch.cat([w_f, w_s], dim=0)                                              # [2F, F_dst + F_src + dim]
+    b = None if b_f is None else torch.cat([b_f, b_s])
+    w_a, w_b = w[:, :fd], w[:, fd:fd + fs]
+    c = None if edge_attr is None else dense.linear(edge_attr, w[:, fd + fs:].contiguous())
+    if isinstance(x, Tensor):
+        b_uv = None if b is None else torch.cat([b, torch.zeros_like(b)])
+        return dense.linear(x, torch.cat([w_a, w_b], dim=0), b_uv), None, c
+    return dense.linear(x_dst, w_a.contiguous(), b), dense.linear(x_src, w_b.contiguous()), c
+
+
+class CGConv(torch.nn.Module):
+    """x_i + AGGR_j sigmoid(z_ij W_f + b_f) * softplus(z_ij W_s + b_s), z_ij = [x_i, x_j, e_ji] (cg_conv.py:12-101),
+    with AGGR = sum (default) or mean and an optional BatchNorm1d before the residual.  The two Linears are split into
+    per-node products and the per-edge c (`cg_uvc`), and the message runs with its aggregation as one sweep
+    (`Fn.aggregate_cg`).  Other aggregations raise ValueError."""
+
+    def __init__(self, channels, dim: int = 0, aggr: str = "add", batch_norm: bool = False, bias: bool = True,
+                 **kwargs):
+        super().__init__()
+        if aggr not in ("add", "sum", "mean"):
+            raise ValueError(f"aggr='{aggr}' is not on the fused path (sum or mean)")
+        self.aggr = "mean" if aggr == "mean" else "sum"
+        self.flow = kwargs.get("flow", "source_to_target")
+        self.channels, self.dim, self.batch_norm = channels, dim, batch_norm
+        ch = (channels, channels) if isinstance(channels, int) else tuple(channels)
+        self.lin_f = _Lin(sum(ch) + dim, ch[1], bias=bias)                        # cg_conv.py:62-67
+        self.lin_s = _Lin(sum(ch) + dim, ch[1], bias=bias)
+        self.bn = torch.nn.BatchNorm1d(ch[1]) if batch_norm else None
+
+    def forward(self, x, edge_index: Adj, edge_attr: Optional[Tensor] = None) -> Tensor:
+        if (edge_attr is not None) != (self.dim > 0):
+            raise ValueError(f"edge_attr must be given exactly when dim > 0 (dim={self.dim})")
+        pair = _pair(x)
+        graph = _plain_graph(edge_index, pair[0].size(0), pair[1].size(0), self.flow)
+        u, v, c = cg_uvc(x if isinstance(x, Tensor) else pair, edge_attr, self.lin_f.weight, self.lin_f.bias,
+                         self.lin_s.weight, self.lin_s.bias)
+        out = Fn.aggregate_cg_uv(graph, u, c, self.aggr) if v is None else Fn.aggregate_cg(graph, u, v, c, self.aggr)
+        if self.bn is not None:
+            out = self.bn(out)
+        return out + pair[1]
+
+    def __repr__(self) -> str:
+        return f"{self.__class__.__name__}({self.channels}, dim={self.dim})"
 
 
 def pna_uv_c(x: Tensor, edge_attr: Optional[Tensor], pre_weights, pre_biases, enc_w: Optional[Tensor],

@@ -498,6 +498,84 @@ def gated_backward_src(rowptr_t: Tensor, col_t: Tensor, val_t: Optional[Tensor],
     return grad_q, grad_v
 
 
+def _cg_rows(u: Tensor, v: Tensor, c: Optional[Tensor], n_edges: int) -> int:
+    """Check the operands of the crystal-graph sweeps; returns F.  u: [n_dst, 2F], v: [n_src, 2F], each with unit
+    feature stride and its own row stride >= 2F; c: None or a contiguous [n_edges, 2F] tensor; one dtype."""
+    if u.dim() != 2 or u.size(1) % 2:
+        raise ValueError(f"u must be a [N, 2F] tensor, got {tuple(u.shape)}")
+    F = u.size(1) // 2
+    for name, t in (("u", u), ("v", v)):
+        if t.dim() != 2 or t.size(1) != 2 * F or t.dtype != u.dtype or (t.size(0) > 0 and t.stride(1) != 1) \
+                or (t.size(0) > 1 and t.stride(0) < 2 * F):
+            raise ValueError(f"{name} must be a [N, {2 * F}] tensor of u's dtype with unit feature stride, "
+                             f"got {tuple(t.shape)} {t.dtype} strides {t.stride()}")
+    if c is not None and (tuple(c.shape) != (n_edges, 2 * F) or c.dtype != u.dtype or not c.is_contiguous()):
+        raise ValueError(f"c must be a contiguous [{n_edges}, {2 * F}] tensor of u's dtype, got {tuple(c.shape)} {c.dtype}")
+    return F
+
+
+def _ld(t: Tensor) -> int:
+    return t.stride(0) if t.size(0) > 1 else t.size(1)
+
+
+def cg_csr(rowptr: Tensor, col: Tensor, perm: Optional[Tensor], u: Tensor, v: Tensor, c: Optional[Tensor],
+           n_rows: int, reduce: str = "sum", plan: Optional[LongRowPlan] = None) -> Tensor:
+    """out[i,:] = REDUCE_{e in row i} sigmoid(f_e) * softplus(s_e) for sum / mean, [f_e | s_e] = u[i] + v[col[e]]
+    (+ c[perm[e]]).  u: [n_rows, 2F], v: [n_src, 2F] (each with its own row stride); c: [E, 2F] in the caller's edge
+    order or None; perm: CSR slot -> caller's edge id, None for an adopted CSR."""
+    _cuda(rowptr, col, perm, u, v, c)
+    if reduce not in ("sum", "add", "mean"):
+        raise ValueError(f"cg_csr reduces by sum or mean, not '{reduce}'")
+    F = _cg_rows(u, v, c, col.numel())
+    it = _same_idx(rowptr, col, perm)
+    out = torch.empty(n_rows, F, dtype=u.dtype, device=u.device)
+    pargs, _ = _plan_args(plan, F, u.device)
+    _timed("cg_csr", 2 if pargs[2] else 1, lib().b200mp_cg_csr, _p(rowptr), _p(col), _p(perm), _p(u), _p(v), _p(c),
+           _p(out), n_rows, v.size(0), col.numel(), F, _ld(u), _ld(v), REDUCE[reduce], *pargs, it, _vdt(u), _stream())
+    return out
+
+
+def cg_backward_dst(rowptr: Tensor, col: Tensor, perm: Optional[Tensor], u: Tensor, v: Tensor, c: Optional[Tensor],
+                    grad_out: Tensor, grad_u: Tensor, want_grad_c: bool, reduce: str = "sum",
+                    plan: Optional[LongRowPlan] = None) -> Optional[Tensor]:
+    """Destination sweep of the crystal-graph backward: writes grad_u[i] = sum_e [df_e | ds_e] into `grad_u` (u's shape
+    and row stride) and, with want_grad_c, returns grad_c [E, 2F] = [df_e | ds_e] in the caller's edge order."""
+    _cuda(rowptr, col, perm, u, v, c, grad_out, grad_u)
+    F = _cg_rows(u, v, c, col.numel())
+    if _cg_rows(grad_u, v, None, 0) != F or grad_u.size(0) != u.size(0) or _ld(grad_u) != _ld(u):
+        raise ValueError("grad_u must have the shape and row stride of u")
+    if want_grad_c and c is None:
+        raise ValueError("grad_c is the gradient of c: want_grad_c needs c")
+    grad_out = grad_out.contiguous()
+    it = _same_idx(rowptr, col, perm)
+    E = col.numel()
+    grad_c = torch.empty(E, 2 * F, dtype=u.dtype, device=u.device) if want_grad_c else None
+    pargs, _ = _plan_args(plan, 2 * F, u.device)
+    _timed("cg_backward_dst", 2 if pargs[2] else 1, lib().b200mp_cg_backward_dst, _p(rowptr), _p(col), _p(perm), _p(u),
+           _p(v), _p(c), _p(grad_out), _p(grad_u), _p(grad_c), u.size(0), v.size(0), E, F, _ld(u), _ld(v),
+           REDUCE[reduce], *pargs, it, _vdt(u), _stream())
+    return grad_c
+
+
+def cg_backward_src(rowptr_t: Tensor, col_t: Tensor, perm_t: Tensor, val_t: Optional[Tensor], u: Tensor, v: Tensor,
+                    c: Optional[Tensor], grad_out: Tensor, grad_v: Tensor,
+                    plan_t: Optional[LongRowPlan] = None) -> Tensor:
+    """Transposed-CSR sweep of the crystal-graph backward: grad_v[j] = sum_t [df_t | ds_t] with g = val_t[t] *
+    grad_out[col_t[t]] (val_t None: 1), written into `grad_v` (v's shape and row stride)."""
+    _cuda(rowptr_t, col_t, perm_t, val_t, u, v, c, grad_out, grad_v)
+    E = col_t.numel()
+    F = _cg_rows(u, v, c, E)
+    if _cg_rows(u, grad_v, None, 0) != F or grad_v.size(0) != v.size(0) or _ld(grad_v) != _ld(v):
+        raise ValueError("grad_v must have the shape and row stride of v")
+    grad_out = grad_out.contiguous()
+    it = _same_idx(rowptr_t, col_t, perm_t)
+    pargs, _ = _plan_args(plan_t, 2 * F, u.device)
+    _timed("cg_backward_src", 2 if pargs[2] else 1, lib().b200mp_cg_backward_src, _p(rowptr_t), _p(col_t), _p(perm_t),
+           _p(val_t), _p(u), _p(v), _p(c), _p(grad_out), _p(grad_v), v.size(0), u.size(0), E, F, _ld(u), _ld(v),
+           *pargs, it, _vdt(u), _stream())
+    return grad_v
+
+
 def scatter_coo(src: Tensor, index: Tensor, n_rows: int, reduce: str = "sum") -> Tensor:
     """Atomic COO fallback for an unsorted index; fp32, src: [E, F]."""
     _cuda(src, index)

@@ -25,6 +25,7 @@ from torch_geometric.typing import (Adj, NoneType, OptPairTensor, OptTensor, Pai
                                     SparseTensor)  # (names the inherited `# propagate_type:` annotations are evaluated with)
 
 from .. import dense
+from .. import functional as Fn
 from .. import utils as U
 from ..graph import CSRGraph, cached_graph
 from ..nn import conv as C
@@ -35,7 +36,7 @@ from ._util import plain
 # Inspector caches class sources by `cls.__name__` (torch_geometric/inspector.py:323-334), so a subclass that reused
 # its parent's name would hide the parent's `# propagate_type:` annotation and get a `propagate` without arguments.
 LAYERS = {n: "B200" + n for n in ("GCNConv", "SAGEConv", "GraphConv", "GINConv", "GATConv", "GATv2Conv", "TransformerConv",
-                                  "RGCNConv", "FastRGCNConv", "PNAConv")}
+                                  "RGCNConv", "FastRGCNConv", "PNAConv", "CGConv")}
 
 
 def _has_hooks(self) -> bool:
@@ -317,4 +318,33 @@ class B200PNAConv(tgnn.PNAConv):
                 # unbind: one [N, T, (1 + A S) F] gradient for all towers, where block[:, t] would allocate one per tower
                 out = torch.cat([nn(b) for nn, b in zip(self.post_nns, block.unbind(1))], dim=1)   # pna_conv.py:170-173
                 return self.lin(out)
+        return super().forward(x, edge_index, edge_attr)
+
+
+def _cg_fusable(self, xs, edge_attr) -> bool:
+    """The fused CGConv path covers sum / mean aggregation, CUDA float32 / bfloat16 inputs with a destination tensor,
+    and edge_attr given exactly when dim > 0 with dim columns (otherwise the reference raises its own error)."""
+    if type(self.aggr_module) not in (tgnn.aggr.SumAggregation, tgnn.aggr.MeanAggregation):
+        return False
+    if xs[1] is None or xs[0].dim() != 2 or xs[1].dim() != 2:
+        return False
+    if (edge_attr is None) != (self.dim == 0):
+        return False
+    if edge_attr is not None and (edge_attr.dim() != 2 or edge_attr.size(1) != self.dim):
+        return False
+    return _fast(self, xs[0], xs[1], edge_attr) and len({t.dtype for t in (xs[0], xs[1], edge_attr) if t is not None}) == 1
+
+
+class B200CGConv(tgnn.CGConv):
+    def forward(self, x, edge_index, edge_attr=None) -> Tensor:
+        xs = _pair(x)
+        if _cg_fusable(self, xs, edge_attr):
+            g = _graph(edge_index, xs[0].size(0), xs[1].size(0), self.flow)
+            if g is not None:
+                reduce = "mean" if type(self.aggr_module) is tgnn.aggr.MeanAggregation else "sum"
+                u, v, c = C.cg_uvc(x if isinstance(x, Tensor) else xs, edge_attr, self.lin_f.weight, self.lin_f.bias,
+                                   self.lin_s.weight, self.lin_s.bias)
+                out = Fn.aggregate_cg_uv(g, u, c, reduce) if v is None else Fn.aggregate_cg(g, u, v, c, reduce)
+                out = out if self.bn is None else self.bn(out)                       # cg_conv.py:86-88
+                return out + xs[1]
         return super().forward(x, edge_index, edge_attr)

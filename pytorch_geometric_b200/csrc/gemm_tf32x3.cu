@@ -5,21 +5,29 @@
 //     gx = g  W        [M,N] x [N,K]          (grad wrt input)
 //     gW = g^T x       [N,M] x [M,K]          (grad wrt weight, reduction over the M = #nodes rows)
 // The reference runs them as strict-fp32 cuBLAS SIMT kernels (allow_tf32=False).  A single-pass TF32
-// GEMM would be much faster but only ~1e-3 accurate, so this kernel uses the error-compensated
-// 3xTF32 split:  a = a_hi + a_lo  (a_hi = rn_tf32(a), a_lo = a - a_hi exactly), and
-//     a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi      (dropped term a_lo*b_lo ~ 2^-22 |a b|)
-// accumulated in fp32 registers -- fp32-class accuracy at a third of the TF32 tensor rate.
+// GEMM would be much faster but only ~1e-3 accurate, so this kernel uses an error-compensated
+// split:  a = a_hi + a_lo  (a_hi = rn_tf32(a), a_lo = a - a_hi exactly, |a_lo| <= 2^-11 |a|), and
+//     a*b ~= [bf16(a_lo)*bf16(b_hi) + bf16(a_hi)*bf16(b_lo)] + a_hi*b_hi      (dropped term a_lo*b_lo ~ 2^-22 |a b|)
+// accumulated in fp32 registers.  The two correction products are 2^-11 of the result, so BF16's 8 significant bits
+// suffice for them (per term at most 2^-17 + 2^-22 of |a b|), and both fit in ONE wgmma k16 BF16 instruction: logical k
+// becomes the bf16 pair (2k, 2k+1) holding (a_lo, a_hi) in A and (b_hi, b_lo) in B.  A k-step of 8 thus costs one BF16
+// and one TF32 MMA of equal issue cost instead of three TF32 ones -- fp32-class accuracy at half the TF32 tensor rate.
+// (The "tf32x3" names of the entry points date from the three-product form.)
 //
 // Structure (one persistent CTA per SM, 384 threads = three warpgroups, 128 x BN output tiles, BK = 32):
 //   warpgroup 0, warp 0   TMA producer: one thread streams the raw fp32 A and B tiles into a ring of shared-memory
 //                         stages (cp.async.bulk.tensor.2d, mbarrier complete_tx)
 //   warpgroup 0, warps 1-3  B preparation, only when B is MN-major or arrives unsplit: split (and transpose) the
-//                         stage's B tile into a 2-slot ring of (hi, lo) K-major 128B-swizzled buffers, one k-block
-//                         ahead of the tensor cores.  A pre-split K-major B (W_hi, W_lo of the forward) is already
-//                         in that layout as TMA writes it: the wgmma descriptors then point at the stage itself.
-//   warpgroups 1-2        consumers, 64 output rows each.  Per k-block they issue 4 k-steps x 3 products of
-//                         wgmma.m64nBNk8.f32.tf32.tf32 (A from registers, B from shared memory) and, while those
-//                         run, load and split the A fragments of the next k-block -- possibly the next tile's --
+//                         stage's B tile into a 2-slot ring of (hi, correction) K-major 128B-swizzled buffers, one
+//                         k-block ahead of the tensor cores.  The correction tile's 32-bit words are
+//                         pack(bf16(b_hi), bf16(b_lo)) at the place of the fp32 element.  A pre-split K-major B
+//                         (W_hi, W_lo of the forward) is packed once per call into a global correction matrix
+//                         (pack_corr_kernel); TMA then writes hi and correction tiles in the wgmma layout, and the
+//                         descriptors point at the stage itself.
+//   warpgroups 1-2        consumers, 64 output rows each.  Per k-block they issue 4 k-steps x (one
+//                         wgmma.m64nBNk16.f32.bf16.bf16 correction, then one wgmma.m64nBNk8.f32.tf32.tf32 hi*hi)
+//                         (A from registers, B from shared memory) and, while those run, load and split the A
+//                         fragments of the next k-block -- possibly the next tile's --
 //                         into the other of two register sets; then wgmma.wait_group 0, and one thread per
 //                         warpgroup releases the stage (and split slot).  (Keeping a group in flight across
 //                         k-blocks with wait_group 1 made ptxas serialize every wgmma: C7518.)
@@ -27,6 +35,8 @@
 // Operands may be K-major (row-major [rows, K]) or MN-major (row-major [K, rows]), so all three products
 // read x, g and W exactly as they lie in HBM (no transposes in global memory).
 #include <cuda.h>
+
+#include <mutex>
 
 #include "common.cuh"
 
@@ -75,6 +85,12 @@ __device__ __forceinline__ float rn_tf32(float a) {
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(a));
     return __uint_as_float(r);
 }
+// bf16 pair (lower half, upper half) = (rn_bf16(lower), rn_bf16(upper)): positions 2k and 2k+1 of a bf16 operand
+__device__ __forceinline__ uint32_t pack_bf16x2(float lower, float upper) {
+    uint32_t r;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(upper), "f"(lower));
+    return r;
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
@@ -84,16 +100,18 @@ __device__ __forceinline__ void fence_regs(float (&d)[R]) {
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// A fragments of one k-block, split: [k-step][register].  Fenced like the accumulators, so that their definitions
-// stay ahead of wgmma.fence and ptxas has no reason to inject warpgroup.arrive inside the MMA window.
+// A fragments of one k-block, split: [k-step][register].  Register i of the m64k8 tf32 fragment holds (row r or r+8,
+// k = t or t+4); register i of the m64k16 bf16 fragment holds the same row at bf16 positions 2k, 2k+1 -- so corr[j][i]
+// = pack(bf16(a_lo), bf16(a_hi)) of the thread's own element i, no shuffles.  Fenced like the accumulators, so that
+// their definitions stay ahead of wgmma.fence and ptxas has no reason to inject warpgroup.arrive inside the MMA window.
 struct AFrag {
-    uint32_t hi[4][4], lo[4][4];
+    uint32_t hi[4][4], corr[4][4];
 };
 __device__ __forceinline__ void fence_frag(AFrag& f) {
 #pragma unroll
     for (int j = 0; j < 4; ++j)
 #pragma unroll
-        for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(f.hi[j][i]), "+r"(f.lo[j][i])::"memory");
+        for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(f.hi[j][i]), "+r"(f.corr[j][i])::"memory");
 }
 
 // d[64 x N] (+)= a[64 x 8] (registers, tf32) . b[8 x N] (shared memory, K-major, tf32)
@@ -123,10 +141,42 @@ __device__ __forceinline__ void wgmma_m64n128k8_tf32_rs(float (&d)[64], const ui
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
         : "memory");
 }
+// d[64 x N] (+)= a[64 x 16] (registers, bf16) . b[16 x N] (shared memory, K-major, bf16; trans-b = 0)
+__device__ __forceinline__ void wgmma_m64n64k16_bf16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %37, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
+        : "memory");
+}
+__device__ __forceinline__ void wgmma_m64n128k16_bf16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %69, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
+        : "memory");
+}
 template <int BN>
 __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
     if constexpr (BN == 64) wgmma_m64n64k8_tf32_rs(d, a, bdesc, scale_d);
     else wgmma_m64n128k8_tf32_rs(d, a, bdesc, scale_d);
+}
+template <int BN>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    if constexpr (BN == 64) wgmma_m64n64k16_bf16_rs(d, a, bdesc, scale_d);
+    else wgmma_m64n128k16_bf16_rs(d, a, bdesc, scale_d);
 }
 
 // Shared-memory matrix descriptor of a K-major 128B-swizzled operand (rows of 128 B = 32 tf32 along K,
@@ -188,8 +238,9 @@ __device__ __forceinline__ bool decode_tile(int w, const GemmArgs& args, const i
     return true;
 }
 
-// Shared-memory plan of one instantiation: a ring of raw stages (A tile, then B: raw, or hi and lo when pre-split)
-// and, when B needs preparing, kSplitSlots split (hi, lo) buffers.  As many stages as fit, up to kMaxStages.
+// Shared-memory plan of one instantiation: a ring of raw stages (A tile, then B: raw, or hi and correction when
+// pre-split K-major, or hi and lo when pre-split MN-major) and, when B needs preparing, kSplitSlots (hi, correction)
+// buffers.  As many stages as fit, up to kMaxStages.
 template <int BN, bool B_MN, bool B_PRE>
 struct GemmPlan {
     static constexpr bool kDirectB = B_PRE && !B_MN;               // wgmma reads B straight from the stage
@@ -204,8 +255,9 @@ struct GemmPlan {
     static_assert(kStages >= 2 && kSmem <= kSmemLimit, "one CTA per SM must fit the 227 KB opt-in shared memory of sm_90");
 };
 
-// A_MN / B_MN: operand is MN-major (stored row-major as [K, MN]); B_PRE: B arrives pre-split (tmap_b_hi,
-// tmap_b_lo), else tmap_b_hi is the raw matrix and the B-preparation warps split it.  An MN-major A arrives as
+// A_MN / B_MN: operand is MN-major (stored row-major as [K, MN]); B_PRE: B arrives pre-split (tmap_b_hi, and tmap_b_lo
+// = the packed correction when K-major, lo when MN-major), else tmap_b_hi is the raw matrix and the B-preparation warps
+// split it.  An MN-major A arrives as
 // four [32 k][32 m] boxes with the 128B swizzle, so the column-wise fragment loads do not collide in one bank.
 template <int BN, bool A_MN, bool B_MN, bool B_PRE, bool GROUPED>
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -220,7 +272,7 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     extern __shared__ __align__(1024) unsigned char gemm_smem[];
     const uint32_t smem_base = (s2u(gemm_smem) + 1023u) & ~1023u;
     unsigned char* smem_gen = gemm_smem + (smem_base - s2u(gemm_smem));
-    const uint32_t split_base = smem_base + kStages * kStageBytes;   // split B slots (K-major, 128B swizzle): hi, lo
+    const uint32_t split_base = smem_base + kStages * kStageBytes;   // prepared B slots (K-major, 128B swizzle): hi, corr
     const uint32_t bars = split_base + Plan::kSplitBytes;
     auto bar_full = [&](int s) { return bars + 8u * s; };
     auto bar_empty = [&](int s) { return bars + 8u * (kStages + s); };
@@ -297,7 +349,9 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
                 }
             }
         } else if (!kDirectB && warp >= 1) {
-            // ===================== B preparation: stage -> split slot (hi, lo), K-major 128B swizzle =====================
+            // ============ B preparation: stage -> prepared slot (hi, corr), K-major 128B swizzle ============
+            // corr word of element (n, k) = pack(bf16(b_hi), bf16(b_lo)) at the byte offset of the fp32 element: a
+            // K-major bf16 row of 128 B holds the 32 logical k as pairs, so hi and corr share swizzle and descriptors.
             const int pt = threadIdx.x - 32;                    // 0 .. 95
             int stage = 0, slot = 0;
             uint32_t phase = 0, sphase = 0;
@@ -311,35 +365,40 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
                     bar_wait(bar_sempty(slot), sphase ^ 1u);
                     const unsigned char* sb = smem_gen + stage * kStageBytes + kABytes;
                     unsigned char* bh = smem_gen + (split_base - smem_base) + slot * 2 * kBBytes;
-                    unsigned char* bl = bh + kBBytes;
+                    unsigned char* bc = bh + kBBytes;
                     if (!B_MN) {
                         // raw TMA tile already has the target layout: element-wise
                         for (uint32_t off = pt * 16u; off < kBBytes; off += kPrepWarps * 32 * 16u) {
                             const float4 v = *reinterpret_cast<const float4*>(sb + off);
                             const float4 h = make_float4(rn_tf32(v.x), rn_tf32(v.y), rn_tf32(v.z), rn_tf32(v.w));
+                            const float4 l = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
                             *reinterpret_cast<float4*>(bh + off) = h;
-                            *reinterpret_cast<float4*>(bl + off) = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
+                            *reinterpret_cast<uint4*>(bc + off) = make_uint4(pack_bf16x2(h.x, l.x), pack_bf16x2(h.y, l.y),
+                                                                             pack_bf16x2(h.z, l.z), pack_bf16x2(h.w, l.w));
                         }
                     } else {
                         // raw tile is [32 k][BN n] (unswizzled): gather 4 consecutive k of one n, store one 16-byte chunk
                         const float* rb = reinterpret_cast<const float*>(sb);
                         for (int idx = pt; idx < BN * 8; idx += kPrepWarps * 32) {
                             const int n = idx % BN, kc = idx / BN;
-                            float h[4], l[4];
+                            float h[4];
+                            uint32_t c[4];
 #pragma unroll
                             for (int i = 0; i < 4; ++i) {
                                 const float v = rb[(4 * kc + i) * BN + n];
+                                float l;
                                 if (B_PRE) {
                                     h[i] = v;
-                                    l[i] = rb[BN * kBK + (4 * kc + i) * BN + n];
+                                    l = rb[BN * kBK + (4 * kc + i) * BN + n];
                                 } else {
                                     h[i] = rn_tf32(v);
-                                    l[i] = v - h[i];
+                                    l = v - h[i];
                                 }
+                                c[i] = pack_bf16x2(h[i], l);
                             }
                             const uint32_t off = sw128_offset(n, 4 * kc);
                             *reinterpret_cast<float4*>(bh + off) = make_float4(h[0], h[1], h[2], h[3]);
-                            *reinterpret_cast<float4*>(bl + off) = make_float4(l[0], l[1], l[2], l[3]);
+                            *reinterpret_cast<uint4*>(bc + off) = make_uint4(c[0], c[1], c[2], c[3]);
                         }
                     }
                     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> wgmma (async proxy) reads
@@ -376,7 +435,7 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
                                      : *reinterpret_cast<const float*>(sa + sw128_offset(r, k));
                 const float h = rn_tf32(v);
                 f.hi[j][i] = __float_as_uint(h);
-                f.lo[j][i] = __float_as_uint(v - h);
+                f.corr[j][i] = pack_bf16x2(v - h, h);
             }
         }
     };
@@ -438,17 +497,15 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
             bar_wait(bar_sfull(slot), sphase);
             b_hi = split_base + slot * 2 * kBBytes;
         }
-        const uint32_t b_lo = b_hi + kBBytes;
-        // 4 k-steps x 3 products, small terms first
+        const uint32_t b_corr = b_hi + kBBytes;
+        // 4 k-steps x (bf16 correction pair, tf32 hi*hi), small terms first; the k16 bf16 step and the k8 tf32 step
+        // both advance 32 B along the swizzle row
         fence_frag(cur);
         wgmma_fence();
 #pragma unroll
         for (int j = 0; j < kBK / 8; ++j) {
-            const uint64_t dh = smem_desc_sw128(b_hi + j * 32u);
-            const uint64_t dl = smem_desc_sw128(b_lo + j * 32u);
-            wgmma_tf32<BN>(acc, cur.lo[j], dh, (kb > kb0 || j > 0) ? 1u : 0u);
-            wgmma_tf32<BN>(acc, cur.hi[j], dl, 1u);
-            wgmma_tf32<BN>(acc, cur.hi[j], dh, 1u);
+            wgmma_bf16<BN>(acc, cur.corr[j], smem_desc_sw128(b_corr + j * 32u), (kb > kb0 || j > 0) ? 1u : 0u);
+            wgmma_tf32<BN>(acc, cur.hi[j], smem_desc_sw128(b_hi + j * 32u), 1u);
         }
         wgmma_commit();
         const int cur_stage = stage, cur_slot = slot;
@@ -490,6 +547,11 @@ __global__ void split_tf32_kernel(const float* __restrict__ w, float* __restrict
         hi[i] = h;
         lo[i] = v - h;
     }
+}
+// (hi, lo) -> pack(bf16(hi), bf16(lo)): the correction operand of a pre-split K-major B, element for element
+__global__ void pack_corr_kernel(const float* __restrict__ hi, const float* __restrict__ lo, uint32_t* __restrict__ corr, int64_t n) {
+    const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i < n) corr[i] = pack_bf16x2(hi[i], lo[i]);
 }
 // w [rows, cols] -> (rn_tf32(w^T), w^T - rn_tf32(w^T)) [cols, rows], through a 32 x 32 shared-memory tile
 __global__ void split_tf32_transposed_kernel(const float* __restrict__ w, float* __restrict__ hi, float* __restrict__ lo,
@@ -586,6 +648,51 @@ static int launch_bn(int bn, const CUtensorMap& ta, const CUtensorMap& ta2, cons
                     : launch_gemm<128, A_MN, B_MN, B_PRE>(ta, ta2, tbh, tbl, args, n_work, s);
 }
 
+// Correction operand of a pre-split K-major B, packed once per call from (b_hi, b_lo) into stream-ordered scratch, so
+// that TMA can stage it next to hi with no preparation pass in the kernel.  Freed in stream order when it goes out of
+// scope, after the launch that reads it.  The scratch comes from a memory pool of the library's own per device that
+// keeps what it has mapped (the default pool would hand memory back at every synchronisation and map it again on the
+// next call, which stalls the stream for milliseconds).
+static cudaMemPool_t corr_pool(int dev) {
+    static std::mutex mu;
+    static cudaMemPool_t pools[64] = {};
+    std::lock_guard<std::mutex> lock(mu);
+    if (dev < 0 || dev >= 64) return nullptr;
+    if (!pools[dev]) {
+        cudaMemPoolProps props = {};
+        props.allocType = cudaMemAllocationTypePinned;
+        props.location.type = cudaMemLocationTypeDevice;
+        props.location.id = dev;
+        cudaMemPool_t pool = nullptr;
+        if (cudaMemPoolCreate(&pool, &props) != cudaSuccess) return nullptr;
+        uint64_t keep = UINT64_MAX;
+        cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+        pools[dev] = pool;
+    }
+    return pools[dev];
+}
+struct CorrB {
+    uint32_t* p = nullptr;
+    cudaStream_t s = nullptr;
+    ~CorrB() {
+        if (p) cudaFreeAsync(p, s);
+    }
+};
+static int pack_corr(const float* hi, const float* lo, int64_t n, cudaStream_t s, CorrB& out) {
+    out.s = s;
+    int dev = 0;
+    B200MP_CUDA(cudaGetDevice(&dev));
+    cudaMemPool_t pool = corr_pool(dev);
+    if (!pool) {
+        set_error("gemm: cannot create the correction-operand memory pool on device %d", dev);
+        return B200MP_ERR_CUDA;
+    }
+    B200MP_CUDA(cudaMallocFromPoolAsync(reinterpret_cast<void**>(&out.p), static_cast<size_t>(n) * 4, pool, s));
+    pack_corr_kernel<<<static_cast<unsigned>(ceil_div(n, 256)), 256, 0, s>>>(hi, lo, out.p, n);
+    B200MP_LAUNCH_CHECK();
+    return B200MP_OK;
+}
+
 static bool ok16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 static bool width_ok(int64_t w) { return w == 64 || w == 128 || (w > 0 && w % 256 == 0); }
 static int tile_n(int64_t w) { return w == 64 ? 64 : 128; }
@@ -599,10 +706,16 @@ static int run_pair(const float* a1, int64_t k1, const float* a2, int64_t k2, co
     const int bn = (n1 == 64 && n2 == 0) ? 64 : 128;
     CUtensorMap ta, ta2, tbh, tbl;
     int rc;
+    CorrB corr;
+    const float* b_second = b_lo ? b_lo : b_hi;                 // K-major pre-split: the packed correction, else lo / raw
+    if (b_lo && !b_mn) {
+        if ((rc = pack_corr(b_hi, b_lo, b_rows * b_cols, s, corr))) return rc;
+        b_second = reinterpret_cast<const float*>(corr.p);
+    }
     if ((rc = make_map(&ta, a1, m, k1, k1, false, kBM))) return rc;
     if ((rc = make_map(&ta2, a2 ? a2 : a1, m, a2 ? k2 : k1, a2 ? k2 : k1, false, kBM))) return rc;
     if ((rc = make_map(&tbh, b_hi, b_rows, b_cols, b_cols, b_mn, bn))) return rc;
-    if ((rc = make_map(&tbl, b_lo ? b_lo : b_hi, b_rows, b_cols, b_cols, b_mn, bn))) return rc;
+    if ((rc = make_map(&tbl, b_second, b_rows, b_cols, b_cols, b_mn, bn))) return rc;
     const int kb = static_cast<int>(k_red / kBK);
     GemmArgs args{};
     args.c = c1;
@@ -759,11 +872,18 @@ extern "C" int b200mp_segment_matmul_tf32x3(const float* a, const int64_t* ptr, 
     }
     const bool b_mn = b_layout == 1;                       // 1: B_r = w[r] [K, N] row-major (out = a w[r]); 0: B_r = w[r] [N, K] (out = a w[r]^T)
     const int64_t b_rows = n_seg * (b_mn ? k : n), b_cols = b_mn ? n : k;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
     CUtensorMap ta, tbh, tbl;
     int rc;
+    CorrB corr;
+    const float* b_second = b_lo;                               // layout 0 (K-major): the packed correction
+    if (!b_mn) {
+        if ((rc = pack_corr(b_hi, b_lo, b_rows * b_cols, s, corr))) return rc;
+        b_second = reinterpret_cast<const float*>(corr.p);
+    }
     if ((rc = make_map(&ta, a, m, k, k, false, kBM))) return rc;
     if ((rc = make_map(&tbh, b_hi, b_rows, b_cols, b_cols, b_mn, 128))) return rc;
-    if ((rc = make_map(&tbl, b_lo, b_rows, b_cols, b_cols, b_mn, 128))) return rc;
+    if ((rc = make_map(&tbl, b_second, b_rows, b_cols, b_cols, b_mn, 128))) return rc;
     const int kb = static_cast<int>(k / kBK);
     GemmArgs args{};
     args.c = c;
@@ -777,7 +897,6 @@ extern "C" int b200mp_segment_matmul_tf32x3(const float* a, const int64_t* ptr, 
     args.b_seg_rows = static_cast<int>(b_mn ? k : n);
     // upper bound of the work list: every segment adds at most one partial tile
     const int n_work = static_cast<int>((ceil_div(m, kBM) + n_seg) * args.n_tiles_n);
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
     return b_mn ? launch_gemm<128, false, true, true, true>(ta, ta, tbh, tbl, args, n_work, s)
                 : launch_gemm<128, false, false, true, true>(ta, ta, tbh, tbl, args, n_work, s);
 }

@@ -3,7 +3,9 @@
 Two back ends, same fp32-level accuracy:
   * "tf32x3" (default on shapes it supports): the hand-written wgmma/TMA 3xTF32 GEMMs of
     csrc/gemm_tf32x3.cu -- forward, grad-input and the split-K grad-weight product all read x, g
-    and W exactly as they lie in HBM;
+    and W exactly as they lie in HBM; each k-step issues the two correction products of the split as
+    one BF16 MMA (bf16(a_lo) bf16(b_hi) + bf16(a_hi) bf16(b_lo)) next to the TF32 a_hi b_hi, still
+    fp32-class (at most 2^-17 + 2^-22 of |a b| per term);
   * "cublas": torch.nn.functional.linear in strict fp32 (what the reference runs) -- used for
     shapes outside the kernel's limits (reduction dim % 32, output width in {64,128,256k}) and for
     non-fp32 inputs.  A plain library GEMM, not a fallback of the aggregation path.

@@ -310,6 +310,54 @@ int b200mp_cg_backward_src(const void* rowptr_t, const void* col_t, const void* 
                            int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials,
                            int idx_dtype, int val_dtype, void* stream);
 
+/* ------------------------------------------------------------------ softmax aggregation (online softmax, one sweep)
+ * Per destination i, feature f, in-edge e = (j -> i) in [rowptr[i], rowptr[i+1]), eid(e) = perm[e] or e (perm NULL):
+ *   s_e = x[col[e]] + edge_rows[eid(e)] (rounded) | x[col[e]] | edge_rows[eid(e)]
+ *   m_e = relu(s_e) + eps (message 1: each step rounded, relu keeps NaN)  |  s_e (message 0)
+ *   z_e = t * m_e rounded (t_mode 1: t[0], 2: t[f]) | m_e (t_mode 0)
+ *   out[i, f] = sum_e exp(z_e - M) m_e / (sum_e exp(z_e - M) + 1e-16),  M = max_e z_e;  0 for an empty row
+ * Replaces: SoftmaxAggregation.forward (nn/aggr/basic.py:196-215) with utils/_softmax.py:60-92 (scatter max, exp,
+ * scatter sum, divide, multiply, scatter sum: six [E, F] passes), and GENConv.message (nn/conv/gen_conv.py:231-239).
+ * message 1 needs x (edge_rows optional); message 0 takes exactly one of x and edge_rows.  t: [1] or [feat] fp32
+ * (read on the device: a learnable t costs no host read; t * m is formed in fp32 and rounded to val_dtype).  x: [n_cols, feat]; edge_rows: [n_edges, feat] in
+ * the CALLER's edge order; out: [n_rows, feat]; lse: NULL or [n_rows, feat] fp32 = M + log(S + 1e-16), the only state
+ * the backward needs (NaN where M = +inf: the reference's inf - inf).  One exponential per (edge, feature) by a running
+ * (M, S, A); fp32 accumulation.  Long rows: plan as in b200mp_spmm_csr, partials [n_chunks, 3 feat] fp32, merged in
+ * chunk order by a second launch. */
+int b200mp_softmax_aggr_csr(const void* rowptr, const void* col, const void* perm, const void* x,
+                            const void* edge_rows, const float* t, void* out, float* lse, int64_t n_rows,
+                            int64_t n_cols, int64_t n_edges, int64_t feat, int message, float eps, int t_mode,
+                            const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows,
+                            int64_t n_chunks, int64_t chunk, float* partials, int idx_dtype, int val_dtype,
+                            void* stream);
+/* fp32 workspace elements b200mp_softmax_aggr_backward_dst needs for grad_t. */
+int64_t b200mp_softmax_aggr_workspace(int64_t n_rows, int64_t n_chunks, int64_t feat);
+/* Destination sweep of the backward (replaces the autograd of basic.py:196-215 / _softmax.py:60-92 / gen_conv.py:231-239
+ * over [E, F]).  Recomputes m, z and p_e = exp(z_e - lse_i); with g = grad_out[i], o = out[i]:
+ *   grad_m_e = g p_e (1 + t (m_e - o))   (semi_grad: g p_e)        grad_s_e = grad_m_e [s_e > 0 or NaN] (message 1)
+ *   grad_edge_rows[eid(e)] = grad_s_e  (NULL: not written)          grad_t[f] = sum_i sum_e g p_e m_e (m_e - o)
+ * grad_t: NULL or [feat] fp32 (per-channel sums; the caller sums them for a scalar t), from per-CTA partials folded
+ * in fixed order by b200mp_column_sum in `workspace` (b200mp_softmax_aggr_workspace elements).  The 1e-16 of the
+ * forward's denominator is dropped here: the denominator is >= 1, so it is below fp32 resolution. */
+int b200mp_softmax_aggr_backward_dst(const void* rowptr, const void* col, const void* perm, const void* x,
+                                     const void* edge_rows, const float* t, const void* out, const float* lse,
+                                     const void* grad_out, void* grad_edge_rows, float* grad_t, float* workspace,
+                                     int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t feat, int message,
+                                     float eps, int t_mode, int semi_grad, const int64_t* long_rows,
+                                     const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks, int64_t chunk,
+                                     int idx_dtype, int val_dtype, void* stream);
+/* grad_x by ONE sweep over the TRANSPOSED CSR: grad_x[j] = sum_{t in rowT(j)} grad_s_t, gathering grad_out, out and
+ * lse of col_t[t] and edge_rows[perm_t[t]] (frozen edge rows) per out-edge.  Needs x.  Used when no grad_edge_rows
+ * was written; otherwise the segment sum of grad_edge_rows over the transposed CSR (b200mp_spmm_csr with perm_t as
+ * the column) gives grad_x with fewer bytes.  Long source rows: the transposed CSR's plan, partials [n_chunks, feat]. */
+int b200mp_softmax_aggr_backward_src(const void* rowptr_t, const void* col_t, const void* perm_t, const void* x,
+                                     const void* edge_rows, const float* t, const void* out, const float* lse,
+                                     const void* grad_out, void* grad_x, int64_t n_src, int64_t n_dst,
+                                     int64_t n_edges, int64_t feat, int message, float eps, int t_mode,
+                                     int semi_grad, const int64_t* long_rows, const int64_t* chunk_ptr,
+                                     int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials,
+                                     int idx_dtype, int val_dtype, void* stream);
+
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)
  * out[index[e], :] (+)= src[e, :] for an UNSORTED index.  Replaces utils/_scatter.py:14-138
  * (aten::scatter_add_ / scatter_reduce_, torch_scatter.scatter).  fp32 only.  `count` is a

@@ -52,6 +52,13 @@ _SIGS = {
     "b200mp_cg_csr": (_INT, [_P] * 7 + [_I64] * 6 + [_INT, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
     "b200mp_cg_backward_dst": (_INT, [_P] * 9 + [_I64] * 6 + [_INT, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
     "b200mp_cg_backward_src": (_INT, [_P] * 9 + [_I64] * 6 + [_P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
+    "b200mp_softmax_aggr_csr": (_INT, [_P] * 8 + [_I64] * 4 + [_INT, _F, _INT, _P, _P, _I64, _I64, _I64, _P, _INT, _INT,
+                                                                _P]),
+    "b200mp_softmax_aggr_workspace": (_I64, [_I64, _I64, _I64]),
+    "b200mp_softmax_aggr_backward_dst": (_INT, [_P] * 12 + [_I64] * 4 + [_INT, _F, _INT, _INT, _P, _P, _I64, _I64, _I64,
+                                                                           _INT, _INT, _P]),
+    "b200mp_softmax_aggr_backward_src": (_INT, [_P] * 10 + [_I64] * 4 + [_INT, _F, _INT, _INT, _P, _P, _I64, _I64, _I64,
+                                                                           _P, _INT, _INT, _P]),
     "b200mp_scatter_coo": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
     "b200mp_split_tf32": (_INT, [_P, _P, _P, _I64, _P]),
     "b200mp_split_tf32_transposed": (_INT, [_P, _P, _P, _I64, _I64, _P]),

@@ -296,6 +296,83 @@ def aggregate_cg_uv(graph: CSRGraph, uv: Tensor, c: Optional[Tensor] = None, red
                               "mean" if reduce == "mean" else "sum")
 
 
+class _SoftmaxAggregate(torch.autograd.Function):
+    """sum_e softmax_e(t * m_e) * m_e per destination and feature (csrc/softmax_aggr.cu).  The only saved state is
+    the fp32 lse plane; the backward recomputes m, z and p.  The destination sweep gives grad_a and grad_t; grad_x is
+    then the segment sum of grad_a's rows over the transposed CSR, and otherwise one transposed sweep.  Each sweep runs
+    only when one of its outputs is needed."""
+
+    @staticmethod
+    def forward(ctx, x, a, t, where, eps: float, message: str, semi_grad: bool, want_lse: bool):
+        rowptr, col, perm, plan, n_edges, _ = where
+        out, lse = ops.softmax_aggr_csr(rowptr, col, perm, x, a, t, rowptr.numel() - 1, n_edges, message, eps, plan,
+                                        want_lse)
+        ctx.where, ctx.eps, ctx.message, ctx.semi = where, eps, message, semi_grad
+        ctx.save_for_backward(x, a, t, out, lse)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out: Tensor):
+        x, a, t, out, lse = ctx.saved_tensors
+        rowptr, col, perm, plan, n_edges, graph = ctx.where
+        need_x, need_a, need_t = ctx.needs_input_grad[:3]
+        need_t = need_t and not ctx.semi
+        gx = ga = gt = None
+        if need_a or need_t:
+            ga, gt = ops.softmax_aggr_backward_dst(rowptr, col, perm, x, a, t, out, lse, grad_out, n_edges, ctx.message,
+                                                   ctx.eps, ctx.semi, need_a, need_t, plan)
+            if gt is not None:
+                gt = gt.sum().view(1) if t.numel() == 1 else gt
+        if need_x:
+            graph.build_transpose()
+            if ga is not None:
+                # grad_x[j] = the sum of grad_a over j's out-edges: perm_t is the caller's edge id of each transposed slot
+                gx = ops.spmm_csr(graph.rowptr_t, graph.perm_t, None, ga, graph.num_src, "sum", graph.plan_t)
+            else:
+                gx = ops.softmax_aggr_backward_src(graph.rowptr_t, graph.col_t, graph.perm_t, x, a, t, out, lse,
+                                                   grad_out, ctx.message, ctx.eps, ctx.semi, graph.plan_t)
+        return gx, ga, gt, None, None, None, None, None
+
+
+def softmax_aggregate(graph, x: Optional[Tensor], a: Optional[Tensor] = None, t=1.0, eps: float = 0.0,
+                      message: str = "identity", semi_grad: bool = False) -> Tensor:
+    """SoftmaxAggregation (nn/aggr/basic.py:196-215, utils/_softmax.py:60-92), optionally behind GENConv's message
+    relu(x_j + e_ji) + eps (gen_conv.py:231-239), in one online-softmax sweep with nothing stored per edge:
+
+        m_e = x[j] | a[e] | relu(x[j] (+ a[e])) + eps,   out[i] = sum_{e = (j -> i)} softmax_e(t * m_e) * m_e
+
+    graph: a CSRGraph (x: [num_src, F] gathered per edge; a: [E, F] in the caller's edge order), or (ptr, plan) for a
+    destination-sorted [E, F] message matrix `a` (x None).  message: "identity" (exactly one of x, a) or "relu_eps"
+    (x, a optional).  t: a Python number (1 skips the multiply, as the reference does) or a tensor of 1 or F elements
+    whose values the kernel reads on the device in fp32, so a learnable t adds no host sync; t * m is formed in fp32
+    and rounded to the messages' dtype, and t's gradient has t's shape and dtype.  semi_grad: the softmax
+    weights carry no gradient (t gets none).  Empty rows give 0."""
+    if isinstance(graph, CSRGraph):
+        where = (graph.rowptr, graph.col, graph.perm, graph.plan, graph.num_edges, graph)
+        if x is not None and x.size(0) != graph.num_src:
+            raise ValueError(f"x has {x.size(0)} rows but the graph has {graph.num_src} source nodes")
+    else:
+        if x is not None:
+            raise ValueError("a (ptr, plan) message layout takes the messages as `a`, not x")
+        ptr, plan = graph
+        where = (ptr, None, None, plan, a.size(0), None)
+    ref = x if x is not None else a
+    if ref is None or ref.dim() != 2:
+        raise ValueError("softmax_aggregate takes two-dimensional x or a")
+    if isinstance(t, Tensor):
+        tt = t.reshape(-1).float().contiguous()
+        if tt.numel() not in (1, ref.size(1)):
+            raise ValueError(f"t must have 1 or {ref.size(1)} elements, got {t.numel()}")
+    elif float(t) == 1.0:
+        tt = None                                                          # basic.py:207: no multiply
+    else:
+        tt = torch.full((1, ), float(t), dtype=torch.float32, device=ref.device)   # ATen's fp32 scalar
+    x = None if x is None else x.contiguous()
+    a = None if a is None else a.contiguous()
+    want_lse = torch.is_grad_enabled() and any(v is not None and v.requires_grad for v in (x, a, tt))
+    return _SoftmaxAggregate.apply(x, a, tt, where, float(eps), message, bool(semi_grad), want_lse)
+
+
 class _PNAAggregate(torch.autograd.Function):
     """PNAConv's aggregation of m_e = u_i + w_e, w_e = v_j (+ c_e) (csrc/pna.cu).  The sweep collects the statistics
     of w (b200mp_multi_aggr_csr on v, or b200mp_pna_edge_stats with c); the epilogue shifts them by u, applies the

@@ -83,32 +83,84 @@ class MinAggregation(Aggregation):
 
 
 class SoftmaxAggregation(Aggregation):
-    """alpha = softmax(t * x) per group; out = sum(alpha * x)   (nn/aggr/basic.py:142-218)."""
+    """alpha = softmax(t * x) per group; out = sum(alpha * x)   (nn/aggr/basic.py:142-218), as one online-softmax
+    sweep over the messages (functional.softmax_aggregate): no [E, F] intermediate is stored, and a learnable t is
+    read on the device."""
 
     def __init__(self, t: float = 1.0, learn: bool = False, semi_grad: bool = False, channels: int = 1):
         super().__init__()
         if learn and semi_grad:
-            raise ValueError("Cannot enable 'semi_grad' if 't' is learnable")
+            raise ValueError(f"Cannot enable 'semi_grad' in '{self.__class__.__name__}' in case the temperature term "
+                             f"'t' is learnable")
+        if not learn and channels != 1:
+            raise ValueError(f"Cannot set 'channels' greater than '1' in case '{self.__class__.__name__}' is not "
+                             f"trainable")
         self._init_t = t
         self.learn, self.semi_grad, self.channels = learn, semi_grad, channels
-        self.t = torch.nn.Parameter(torch.full((channels, ), float(t))) if learn else t
+        self.t = torch.nn.Parameter(torch.empty(channels)) if learn else t
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        if isinstance(self.t, Tensor):
+            self.t.data.fill_(self._init_t)
 
     def forward(self, x, index=None, ptr=None, dim_size=None, dim=-2, index_sorted=False):
+        d = dim + x.dim() if dim < 0 else dim
+        if self.channels != 1:                                           # base.py:162-169
+            if x.dim() != 2:
+                raise ValueError(f"Aggregation requires two-dimensional inputs (got '{x.dim()}')")
+            if dim not in (-2, 0):
+                raise ValueError(f"Aggregation needs to perform aggregation in first dimension (got '{dim}')")
+        if not _softmax_fusable(x, self.t):
+            return self._composed(x, index, ptr, dim_size, d, index_sorted)
+        # the aggregated dimension first, every other one folded into the feature width (t broadcasts over the last)
+        xm = x.movedim(d, 0)
+        rest = xm.shape[1:]
+        x2 = xm.reshape(xm.size(0), -1)
+        out = _softmax_forward(x2, self.t, self.semi_grad and not self.learn, index, ptr, dim_size, index_sorted)
+        return out.view(out.size(0), *rest).movedim(0, d)
+
+    def _composed(self, x, index, ptr, dim_size, d, index_sorted):
+        """The reference's op sequence (basic.py:196-215) on the engine's softmax and scatter, which compute in fp32:
+        for messages the fused sweep does not take (fp16, fp64), and for a t whose dtype differs from the messages',
+        where x * t promotes and the result takes the promoted dtype."""
         t = self.t
         if self.channels != 1:
-            shape = [1] * x.dim()
-            shape[-1] = -1
-            t = t.view(shape)
+            t = t.view(-1, self.channels)
         alpha = x
         if not isinstance(t, (int, float)) or t != 1:
             alpha = x * t
-        d = dim + x.dim() if dim < 0 else dim
         if not self.learn and self.semi_grad:
             with torch.no_grad():
                 alpha = U.softmax(alpha, index, ptr, dim_size, d)
         else:
             alpha = U.softmax(alpha, index, ptr, dim_size, d)
-        return self.reduce(x * alpha, index, ptr, dim_size, dim, "sum", index_sorted)
+        return self.reduce(x * alpha, index, ptr, dim_size, d, "sum", index_sorted)
+
+    def __repr__(self) -> str:
+        return f"{self.__class__.__name__}(learn={self.learn})"
+
+
+def _softmax_fusable(x: Tensor, t) -> bool:
+    """The fused sweep takes CUDA float32 / bfloat16 messages, with a Python-number t or a t of the messages' dtype."""
+    return x.is_cuda and x.dtype in (torch.float32, torch.bfloat16) and (not isinstance(t, Tensor) or t.dtype == x.dtype)
+
+
+def _softmax_forward(x, t, semi_grad, index, ptr, dim_size, index_sorted):
+    """softmax_aggregate over a [E, F] message matrix, grouped by ptr or index (as _fused_forward groups them)."""
+    if ptr is None and index is None:
+        raise NotImplementedError("Aggregation requires 'index' to be specified")
+    if x.size(0) == 0:
+        n = dim_size if dim_size is not None else (ptr.numel() - 1 if ptr is not None else 0)
+        return x.new_zeros(n, x.size(1))
+    if ptr is None and index_sorted:
+        ptr = ops.index2ptr(index, dim_size)
+    if ptr is not None:
+        return Fn.softmax_aggregate((ptr, ops.segment_plan(ptr, x.size(0))), None, x, t, semi_grad=semi_grad)
+    # unsorted index: a CSR over the messages themselves; the sweep reads message perm[e] of CSR slot e in place
+    from ..graph import CSRGraph
+    e = torch.arange(index.numel(), device=index.device, dtype=index.dtype)
+    return Fn.softmax_aggregate(CSRGraph(e, index, index.numel(), dim_size), None, x, t, semi_grad=semi_grad)
 
 
 class VarAggregation(Aggregation):

@@ -576,6 +576,99 @@ def cg_backward_src(rowptr_t: Tensor, col_t: Tensor, perm_t: Tensor, val_t: Opti
     return grad_v
 
 
+SOFTMAX_MESSAGES = {"identity": 0, "relu_eps": 1}
+
+
+def _softmax_aggr_args(x: Optional[Tensor], a: Optional[Tensor], t: Optional[Tensor], message: str, n_edges: int):
+    """Check the operands of the softmax-aggregation sweeps; returns (F, message code, t_mode).  x: [n_src, F] or
+    None; a: [n_edges, F] in the caller's edge order or None, contiguous, one dtype; t: None or fp32 [1] / [F]."""
+    if message not in SOFTMAX_MESSAGES:
+        raise ValueError(f"message must be one of {sorted(SOFTMAX_MESSAGES)}, got '{message}'")
+    if message == "relu_eps" and x is None:
+        raise ValueError("the relu_eps message needs x")
+    if message == "identity" and (x is None) == (a is None):
+        raise ValueError("the identity message takes exactly one of x and the edge rows")
+    ref = x if x is not None else a
+    F = ref.size(1)
+    for name, v in (("x", x), ("edge rows", a)):
+        if v is not None and (v.dim() != 2 or v.size(1) != F or v.dtype != ref.dtype or not v.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous [N, {F}] tensor of dtype {ref.dtype}, got {tuple(v.shape)}")
+    if a is not None and a.size(0) != n_edges:
+        raise ValueError(f"edge rows must have {n_edges} rows, got {a.size(0)}")
+    t_mode = 0
+    if t is not None:
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() not in (1, F):
+            raise ValueError(f"t must be a contiguous float32 tensor of 1 or {F} elements, got {tuple(t.shape)} {t.dtype}")
+        t_mode = 1 if t.numel() == 1 else 2
+    return F, SOFTMAX_MESSAGES[message], t_mode
+
+
+def softmax_aggr_csr(rowptr: Tensor, col: Optional[Tensor], perm: Optional[Tensor], x: Optional[Tensor],
+                     a: Optional[Tensor], t: Optional[Tensor], n_rows: int, n_edges: int, message: str = "identity",
+                     eps: float = 0.0, plan: Optional[LongRowPlan] = None,
+                     want_lse: bool = False) -> Tuple[Tensor, Optional[Tensor]]:
+    """out[i] = sum_e softmax_e(t * m_e) m_e over row i (b200mp_softmax_aggr_csr), m_e = x[col[e]] / a[perm[e]] /
+    relu(x[col[e]] (+ a[perm[e]])) + eps; with want_lse also the fp32 lse plane the backward reads."""
+    _cuda(rowptr, col, perm, x, a, t)
+    F, msg, t_mode = _softmax_aggr_args(x, a, t, message, n_edges)
+    it = _same_idx(rowptr, col, perm)
+    ref = x if x is not None else a
+    out = torch.empty(n_rows, F, dtype=ref.dtype, device=ref.device)
+    lse = torch.empty(n_rows, F, dtype=torch.float32, device=ref.device) if want_lse else None
+    pargs, _ = _plan_args(plan, 3 * F, ref.device)
+    _timed("softmax_aggr_csr", 2 if pargs[2] else 1, lib().b200mp_softmax_aggr_csr, _p(rowptr), _p(col), _p(perm),
+           _p(x), _p(a), _p(t), _p(out), _p(lse), n_rows, 0 if x is None else x.size(0), n_edges, F, msg, float(eps),
+           t_mode, *pargs, it, _vdt(ref), _stream())
+    return out, lse
+
+
+def softmax_aggr_backward_dst(rowptr: Tensor, col: Optional[Tensor], perm: Optional[Tensor], x: Optional[Tensor],
+                              a: Optional[Tensor], t: Optional[Tensor], out: Tensor, lse: Tensor, grad_out: Tensor,
+                              n_edges: int, message: str, eps: float, semi_grad: bool, want_grad_a: bool,
+                              want_grad_t: bool, plan: Optional[LongRowPlan] = None):
+    """Destination sweep of the softmax-aggregation backward: (grad_a [E, F] in the caller's edge order or None,
+    grad_t [F] fp32 per-channel sums or None)."""
+    _cuda(rowptr, col, perm, x, a, t, out, lse, grad_out)
+    F, msg, t_mode = _softmax_aggr_args(x, a, t, message, n_edges)
+    if want_grad_t and t is None:
+        raise ValueError("grad_t needs t")
+    it = _same_idx(rowptr, col, perm)
+    grad_out = grad_out.contiguous()
+    n_rows = rowptr.numel() - 1
+    grad_a = torch.empty(n_edges, F, dtype=out.dtype, device=out.device) if want_grad_a else None
+    grad_t = ws = None
+    n_chunks = plan.n_chunks if plan is not None and plan.n_long else 0
+    if want_grad_t:
+        grad_t = torch.empty(F, dtype=torch.float32, device=out.device)
+        ws = torch.empty(max(int(lib().b200mp_softmax_aggr_workspace(n_rows, n_chunks, F)), 1), dtype=torch.float32,
+                         device=out.device)
+    # the destination sweep only splits long rows (nothing to combine): the plan without partials
+    pargs = _plan_args(None, F, out.device)[0] if not n_chunks else (_p(plan.long_rows), _p(plan.chunk_ptr), plan.n_long,
+                                                                     plan.n_chunks, plan.chunk)
+    _timed("softmax_aggr_backward_dst", 3 if want_grad_t else 1, lib().b200mp_softmax_aggr_backward_dst, _p(rowptr),
+           _p(col), _p(perm), _p(x), _p(a), _p(t), _p(out), _p(lse), _p(grad_out), _p(grad_a), _p(grad_t), _p(ws),
+           n_rows, 0 if x is None else x.size(0), n_edges, F, msg, float(eps), t_mode, int(bool(semi_grad)),
+           *pargs[:5], it, _vdt(out), _stream())
+    return grad_a, grad_t
+
+
+def softmax_aggr_backward_src(rowptr_t: Tensor, col_t: Tensor, perm_t: Tensor, x: Tensor, a: Optional[Tensor],
+                              t: Optional[Tensor], out: Tensor, lse: Tensor, grad_out: Tensor, message: str,
+                              eps: float, semi_grad: bool, plan_t: Optional[LongRowPlan] = None) -> Tensor:
+    """Transposed-CSR sweep of the softmax-aggregation backward: grad_x [n_src, F] (a frozen)."""
+    _cuda(rowptr_t, col_t, perm_t, x, a, t, out, lse, grad_out)
+    E = col_t.numel()
+    F, msg, t_mode = _softmax_aggr_args(x, a, t, message, E)
+    it = _same_idx(rowptr_t, col_t, perm_t)
+    grad_out = grad_out.contiguous()
+    grad_x = torch.empty_like(x)
+    pargs, _ = _plan_args(plan_t, F, x.device)
+    _timed("softmax_aggr_backward_src", 2 if pargs[2] else 1, lib().b200mp_softmax_aggr_backward_src, _p(rowptr_t),
+           _p(col_t), _p(perm_t), _p(x), _p(a), _p(t), _p(out), _p(lse), _p(grad_out), _p(grad_x), x.size(0),
+           out.size(0), E, F, msg, float(eps), t_mode, int(bool(semi_grad)), *pargs, it, _vdt(x), _stream())
+    return grad_x
+
+
 def scatter_coo(src: Tensor, index: Tensor, n_rows: int, reduce: str = "sum") -> Tensor:
     """Atomic COO fallback for an unsorted index; fp32, src: [E, F]."""
     _cuda(src, index)

@@ -1057,17 +1057,6 @@ bool attn_vec_ok(int64_t heads, int64_t chan, const AttnArgs& a, const void* out
     return true;
 }
 
-#define ATTN_BY_SHAPE(LAUNCH)                      \
-    do {                                           \
-        if (n_vec <= 1) { LAUNCH(1, 1); }          \
-        else if (n_vec <= 2) { LAUNCH(2, 1); }     \
-        else if (n_vec <= 4) { LAUNCH(4, 1); }     \
-        else if (n_vec <= 8) { LAUNCH(8, 1); }     \
-        else if (n_vec <= 16) { LAUNCH(16, 1); }   \
-        else if (n_vec <= 32) { LAUNCH(32, 1); }   \
-        else { LAUNCH(32, 2); }                    \
-    } while (0)
-
 template <typename T, typename I, int MODE>
 int attn_forward_typed(const void* rowptr_, const void* col_, AttnArgs a, void* out_, float* row_max, float* row_den,
                        float* alpha_out, int64_t n_rows, int64_t n_edges, LongRowPlan plan, float* part_ms, cudaStream_t s) {
@@ -1077,7 +1066,6 @@ int attn_forward_typed(const void* rowptr_, const void* col_, AttnArgs a, void* 
     const int n_vec = a.n_vec;
     const int64_t items = plan.n_chunks + n_rows;
     const unsigned blocks = static_cast<unsigned>(ceil_div(items, kAttnT / 32));
-#define ATTN_FWD(G_, V_) attn_fwd_kernel<T, I, G_, V_, MODE><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, out, row_max, row_den, n_rows, plan, part_ms)
 #define ATTN_FWD_STAGED(G_) attn_fwd_kernel<T, I, G_, 1, MODE, true><<<blocks, kAttnT, stage_bytes, s>>>(rowptr, col, a, out, row_max, row_den, n_rows, plan, part_ms)
 #define ATTN_FWD_STAGED1(G_) attn_fwd_kernel<T, I, G_, 1, MODE, true, 32><<<static_cast<unsigned>(items), 32, stage_bytes / (kAttnT / 32), s>>>(rowptr, col, a, out, row_max, row_den, n_rows, plan, part_ms)
     // lane-private cp.async slots: 2 iterations x 4 edges x (value (+ key) vector + a_src scalar) per thread
@@ -1085,9 +1073,9 @@ int attn_forward_typed(const void* rowptr_, const void* col_, AttnArgs a, void* 
     bool edge_done = false;
     if constexpr (MODE != ATTN_GAT) {
         if (a.ee) {                                                            // per-edge feature rows: register form
-#define ATTN_FWD_EDGE(G_, V_) attn_fwd_kernel<T, I, G_, V_, MODE, 2><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, out, row_max, row_den, n_rows, plan, part_ms)
-            ATTN_BY_SHAPE(ATTN_FWD_EDGE);
-#undef ATTN_FWD_EDGE
+            lane_group_shape<2>(n_vec, [&](auto G, auto VPL) {
+                attn_fwd_kernel<T, I, G(), VPL(), MODE, 2><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, out, row_max, row_den, n_rows, plan, part_ms);
+            });
             edge_done = true;
         }
     }
@@ -1101,11 +1089,12 @@ int attn_forward_typed(const void* rowptr_, const void* col_, AttnArgs a, void* 
         else if (n_vec <= 16) ATTN_FWD_STAGED(16);
         else ATTN_FWD_STAGED(32);
     } else {
-        ATTN_BY_SHAPE(ATTN_FWD);
+        lane_group_shape<2>(n_vec, [&](auto G, auto VPL) {
+            attn_fwd_kernel<T, I, G(), VPL(), MODE><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, out, row_max, row_den, n_rows, plan, part_ms);
+        });
     }
 #undef ATTN_FWD_STAGED1
 #undef ATTN_FWD_STAGED
-#undef ATTN_FWD
     B200MP_LAUNCH_CHECK();
     if (plan.n_long > 0) {
         attn_combine_kernel<T><<<static_cast<unsigned>(plan.n_long), kCombineT, 0, s>>>(out, row_max, row_den, a.heads, a.chan, plan, part_ms,
@@ -1115,18 +1104,20 @@ int attn_forward_typed(const void* rowptr_, const void* col_, AttnArgs a, void* 
     if (alpha_out && n_edges > 0) {
         LongRowPlan np = plan;
         np.partials = nullptr;
-#define ATTN_ALPHA(G_, V_) attn_bwd_dst_kernel<T, I, G_, V_, MODE, true><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, row_max, row_den, nullptr, nullptr, nullptr, alpha_out, nullptr, nullptr, nullptr, n_rows, np)
-#define ATTN_ALPHA_EDGE(G_, V_) attn_bwd_dst_kernel<T, I, G_, V_, MODE, true, 2><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, row_max, row_den, nullptr, nullptr, nullptr, alpha_out, nullptr, nullptr, nullptr, n_rows, np)
         bool alpha_done = false;
         if constexpr (MODE != ATTN_GAT) {
             if (a.ee) {
-                ATTN_BY_SHAPE(ATTN_ALPHA_EDGE);
+                lane_group_shape<2>(n_vec, [&](auto G, auto VPL) {
+                    attn_bwd_dst_kernel<T, I, G(), VPL(), MODE, true, 2><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, row_max, row_den, nullptr, nullptr, nullptr, alpha_out, nullptr, nullptr, nullptr, n_rows, np);
+                });
                 alpha_done = true;
             }
         }
-        if (!alpha_done) ATTN_BY_SHAPE(ATTN_ALPHA);
-#undef ATTN_ALPHA_EDGE
-#undef ATTN_ALPHA
+        if (!alpha_done) {
+            lane_group_shape<2>(n_vec, [&](auto G, auto VPL) {
+                attn_bwd_dst_kernel<T, I, G(), VPL(), MODE, true><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, row_max, row_den, nullptr, nullptr, nullptr, alpha_out, nullptr, nullptr, nullptr, n_rows, np);
+            });
+        }
         B200MP_LAUNCH_CHECK();
     }
     return B200MP_OK;
@@ -1147,15 +1138,14 @@ int attn_backward_typed(const void* rowptr_, const void* col_, const void* rowpt
         const int64_t items = plan.n_chunks + n_rows;
         unsigned blocks = static_cast<unsigned>(ceil_div(items, kAttnT / 32));
         if (MODE == ATTN_GATV2 && blocks > static_cast<unsigned>(gatt_rows)) blocks = static_cast<unsigned>(gatt_rows);   // persistent
-#define ATTN_DST(G_, V_) attn_bwd_dst_kernel<T, I, G_, V_, MODE, false><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, row_max, row_den, static_cast<const T*>(out), static_cast<const T*>(grad_out), pair, nullptr, static_cast<T*>(grad_q), grad_s_dst, gatt_part, n_rows, plan)
 #define ATTN_DST_STAGED(G_) attn_bwd_dst_kernel<T, I, G_, 1, MODE, false, true><<<blocks, kAttnT, dst_stage, s>>>(rowptr, col, a, row_max, row_den, static_cast<const T*>(out), static_cast<const T*>(grad_out), pair, nullptr, static_cast<T*>(grad_q), grad_s_dst, gatt_part, n_rows, plan)
         const size_t dst_stage = static_cast<size_t>(2) * 4 * kAttnT * ((MODE == ATTN_DOT ? 2 : 1) * 16 + 4);
         bool edge_done = false;
         if constexpr (MODE != ATTN_GAT) {
             if (a.ee) {
-#define ATTN_DST_EDGE(G_, V_) attn_bwd_dst_kernel<T, I, G_, V_, MODE, false, 2><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, row_max, row_den, static_cast<const T*>(out), static_cast<const T*>(grad_out), pair, nullptr, static_cast<T*>(grad_q), grad_s_dst, gatt_part, n_rows, plan)
-                ATTN_BY_SHAPE(ATTN_DST_EDGE);
-#undef ATTN_DST_EDGE
+                lane_group_shape<2>(n_vec, [&](auto G, auto VPL) {
+                    attn_bwd_dst_kernel<T, I, G(), VPL(), MODE, false, 2><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, row_max, row_den, static_cast<const T*>(out), static_cast<const T*>(grad_out), pair, nullptr, static_cast<T*>(grad_q), grad_s_dst, gatt_part, n_rows, plan);
+                });
                 edge_done = true;
             }
         }
@@ -1165,10 +1155,11 @@ int attn_backward_typed(const void* rowptr_, const void* col_, const void* rowpt
             else if (n_vec <= 16) ATTN_DST_STAGED(16);
             else ATTN_DST_STAGED(32);
         } else {
-            ATTN_BY_SHAPE(ATTN_DST);
+            lane_group_shape<2>(n_vec, [&](auto G, auto VPL) {
+                attn_bwd_dst_kernel<T, I, G(), VPL(), MODE, false><<<blocks, kAttnT, 0, s>>>(rowptr, col, a, row_max, row_den, static_cast<const T*>(out), static_cast<const T*>(grad_out), pair, nullptr, static_cast<T*>(grad_q), grad_s_dst, gatt_part, n_rows, plan);
+            });
         }
 #undef ATTN_DST_STAGED
-#undef ATTN_DST
         B200MP_LAUNCH_CHECK();
         if (plan.n_long > 0) {
             if (MODE == ATTN_GAT)
@@ -1187,16 +1178,15 @@ int attn_backward_typed(const void* rowptr_, const void* col_, const void* rowpt
     if (n_src > 0) {
         const int64_t items = plan_t.n_chunks + n_src;
         const unsigned blocks = static_cast<unsigned>(ceil_div(items, kAttnT / 32));
-#define ATTN_SRC(G_, V_) attn_bwd_src_kernel<T, I, G_, V_, MODE><<<blocks, kAttnT, 0, s>>>(static_cast<const I*>(rowptr_t_), static_cast<const I*>(col_t_), static_cast<const I*>(t2csr_), a, static_cast<const T*>(grad_out), pair, static_cast<T*>(grad_v), static_cast<T*>(grad_k), grad_s_src, n_src, plan_t)
 #define ATTN_SRC_STAGED(G_) attn_bwd_src_kernel<T, I, G_, 1, MODE, true><<<blocks, kAttnT, src_stage, s>>>(static_cast<const I*>(rowptr_t_), static_cast<const I*>(col_t_), static_cast<const I*>(t2csr_), a, static_cast<const T*>(grad_out), pair, static_cast<T*>(grad_v), static_cast<T*>(grad_k), grad_s_src, n_src, plan_t)
 #define ATTN_SRC_STAGED1(G_) attn_bwd_src_kernel<T, I, G_, 1, MODE, true, 32><<<static_cast<unsigned>(items), 32, src_stage / (kAttnT / 32), s>>>(static_cast<const I*>(rowptr_t_), static_cast<const I*>(col_t_), static_cast<const I*>(t2csr_), a, static_cast<const T*>(grad_out), pair, static_cast<T*>(grad_v), static_cast<T*>(grad_k), grad_s_src, n_src, plan_t)
         const size_t src_stage = static_cast<size_t>(2) * 4 * kAttnT * ((MODE == ATTN_GAT ? 1 : 2) * 16 + 8);
         bool edge_done = false;
         if constexpr (MODE == ATTN_GATV2) {
             if (a.ee) {                                 // x_l's gradient takes the edges' grad_ee rows instead of recomputing them
-#define ATTN_SRC_EDGE(G_, V_) attn_bwd_src_kernel<T, I, G_, V_, MODE, 2><<<blocks, kAttnT, 0, s>>>(static_cast<const I*>(rowptr_t_), static_cast<const I*>(col_t_), static_cast<const I*>(t2csr_), a, static_cast<const T*>(grad_out), pair, static_cast<T*>(grad_v), static_cast<T*>(grad_k), grad_s_src, n_src, plan_t)
-                ATTN_BY_SHAPE(ATTN_SRC_EDGE);
-#undef ATTN_SRC_EDGE
+                lane_group_shape<2>(n_vec, [&](auto G, auto VPL) {
+                    attn_bwd_src_kernel<T, I, G(), VPL(), MODE, 2><<<blocks, kAttnT, 0, s>>>(static_cast<const I*>(rowptr_t_), static_cast<const I*>(col_t_), static_cast<const I*>(t2csr_), a, static_cast<const T*>(grad_out), pair, static_cast<T*>(grad_v), static_cast<T*>(grad_k), grad_s_src, n_src, plan_t);
+                });
                 edge_done = true;
             }
         }
@@ -1210,11 +1200,12 @@ int attn_backward_typed(const void* rowptr_, const void* col_, const void* rowpt
             else if (n_vec <= 16) ATTN_SRC_STAGED(16);
             else ATTN_SRC_STAGED(32);
         } else {
-            ATTN_BY_SHAPE(ATTN_SRC);
+            lane_group_shape<2>(n_vec, [&](auto G, auto VPL) {
+                attn_bwd_src_kernel<T, I, G(), VPL(), MODE><<<blocks, kAttnT, 0, s>>>(static_cast<const I*>(rowptr_t_), static_cast<const I*>(col_t_), static_cast<const I*>(t2csr_), a, static_cast<const T*>(grad_out), pair, static_cast<T*>(grad_v), static_cast<T*>(grad_k), grad_s_src, n_src, plan_t);
+            });
         }
 #undef ATTN_SRC_STAGED1
 #undef ATTN_SRC_STAGED
-#undef ATTN_SRC
         B200MP_LAUNCH_CHECK();
         if (plan_t.n_long > 0) {
             const int64_t w1 = MODE == ATTN_DOT ? hc : 0, wf = MODE == ATTN_GAT ? a.heads : 0;
@@ -1270,31 +1261,15 @@ int fill_args(AttnArgs& a, int mode, const void* v, const void* k, const void* q
 
 }  // namespace
 
-#define ATTN_DISPATCH(FN, ...)                                                                                           \
-    do {                                                                                                                 \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) {                                                        \
-            if (mode == ATTN_GAT) return FN<float, int32_t, ATTN_GAT>(__VA_ARGS__);                                      \
-            if (mode == ATTN_GATV2) return FN<float, int32_t, ATTN_GATV2>(__VA_ARGS__);                                  \
-            return FN<float, int32_t, ATTN_DOT>(__VA_ARGS__);                                                            \
-        }                                                                                                                \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) {                                                        \
-            if (mode == ATTN_GAT) return FN<float, int64_t, ATTN_GAT>(__VA_ARGS__);                                      \
-            if (mode == ATTN_GATV2) return FN<float, int64_t, ATTN_GATV2>(__VA_ARGS__);                                  \
-            return FN<float, int64_t, ATTN_DOT>(__VA_ARGS__);                                                            \
-        }                                                                                                                \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) {                                                       \
-            if (mode == ATTN_GAT) return FN<__nv_bfloat16, int32_t, ATTN_GAT>(__VA_ARGS__);                              \
-            if (mode == ATTN_GATV2) return FN<__nv_bfloat16, int32_t, ATTN_GATV2>(__VA_ARGS__);                          \
-            return FN<__nv_bfloat16, int32_t, ATTN_DOT>(__VA_ARGS__);                                                    \
-        }                                                                                                                \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) {                                                       \
-            if (mode == ATTN_GAT) return FN<__nv_bfloat16, int64_t, ATTN_GAT>(__VA_ARGS__);                              \
-            if (mode == ATTN_GATV2) return FN<__nv_bfloat16, int64_t, ATTN_GATV2>(__VA_ARGS__);                          \
-            return FN<__nv_bfloat16, int64_t, ATTN_DOT>(__VA_ARGS__);                                                    \
-        }                                                                                                                \
-        set_error("attn: unsupported dtype combination val=%d idx=%d", val_dtype, idx_dtype);                            \
-        return B200MP_ERR_UNSUPPORTED;                                                                                   \
-    } while (0)
+// Calls fn(integral_constant<int, MODE>) for the attention mode (checked by the caller to be one of the three).
+template <typename F>
+int dispatch_attn_mode(int mode, F&& fn) {
+    switch (mode) {
+        case ATTN_GAT: return fn(std::integral_constant<int, ATTN_GAT>{});
+        case ATTN_GATV2: return fn(std::integral_constant<int, ATTN_GATV2>{});
+        default: return fn(std::integral_constant<int, ATTN_DOT>{});
+    }
+}
 
 extern "C" int b200mp_attn_supported(int64_t heads, int64_t chan, int val_dtype) {
     const int64_t es = val_dtype == B200MP_BF16 ? 2 : 4;
@@ -1315,9 +1290,11 @@ extern "C" int b200mp_attn_csr_forward(int mode, const void* rowptr, const void*
                                        int val_dtype, void* stream) {
     B200MP_CHECK_ARG(mode >= ATTN_GAT && mode <= ATTN_DOT);
     B200MP_CHECK_ARG(n_rows >= 0 && n_edges >= 0 && heads > 0 && chan > 0);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, part_acc, true)) return rc;
+    B200MP_CHECK_ARG(n_long_rows == 0 || part_ms);
     if (n_rows == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && out && row_max && row_den && (n_edges == 0 || (col && v)));
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && part_acc && part_ms && chunk > 0));
     AttnArgs a;
     if (fill_args(a, mode, v, k, q, s_src, s_dst, att, s_edge, v_stride, k_stride, q_stride, heads, chan, slope, scale, val_dtype, dropout_p, dropout_seed, edge_feat, nullptr)) {
         set_error("attn forward: operands missing for mode %d (or dropout_p outside [0, 1))", mode);
@@ -1329,9 +1306,13 @@ extern "C" int b200mp_attn_csr_forward(int mode, const void* rowptr, const void*
                   static_cast<long long>(heads), static_cast<long long>(chan));
         return B200MP_ERR_UNSUPPORTED;
     }
-    LongRowPlan plan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, part_acc};
-    ATTN_DISPATCH(attn_forward_typed, rowptr, col, a, out, row_max, row_den, alpha_out, n_rows, n_edges, plan, part_ms,
-                  static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "attn_csr_forward", [&](auto tv, auto ti) {
+        return dispatch_attn_mode(mode, [&](auto m) {
+            return attn_forward_typed<decltype(tv), decltype(ti), m()>(rowptr, col, a, out, row_max, row_den, alpha_out,
+                                                                       n_rows, n_edges, plan, part_ms,
+                                                                       static_cast<cudaStream_t>(stream));
+        });
+    });
 }
 
 extern "C" int64_t b200mp_attn_backward_partial_width(int mode, int64_t heads, int64_t chan, int transposed) {
@@ -1363,8 +1344,9 @@ extern "C" int b200mp_attn_csr_backward(int mode, const void* rowptr, const void
     B200MP_CHECK_ARG(mode == ATTN_GAT || grad_q);
     B200MP_CHECK_ARG(mode != ATTN_DOT || grad_k);
     B200MP_CHECK_ARG(mode != ATTN_GATV2 || (grad_att && gatt_part));
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && partials && chunk > 0));
-    B200MP_CHECK_ARG(n_long_rows_t == 0 || (long_rows_t && chunk_ptr_t && partials_t && chunk > 0));
+    LongRowPlan plan, plan_t;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
+    if (int rc = make_plan(plan_t, long_rows_t, chunk_ptr_t, n_long_rows_t, n_chunks_t, chunk, partials_t, true)) return rc;
     AttnArgs a;
     if (fill_args(a, mode, v, k, q, s_src, s_dst, att, s_edge, v_stride, k_stride, q_stride, heads, chan, slope, scale, val_dtype, dropout_p, dropout_seed, edge_feat, grad_edge_feat)) {
         set_error("attn backward: operands missing for mode %d (or dropout_p outside [0, 1))", mode);
@@ -1375,9 +1357,12 @@ extern "C" int b200mp_attn_csr_backward(int mode, const void* rowptr, const void
         set_error("attn backward: shape H=%lld C=%lld not on the vector path", static_cast<long long>(heads), static_cast<long long>(chan));
         return B200MP_ERR_UNSUPPORTED;
     }
-    LongRowPlan plan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, partials};
-    LongRowPlan plan_t{long_rows_t, chunk_ptr_t, n_long_rows_t, n_long_rows_t ? n_chunks_t : 0, chunk, partials_t};
-    ATTN_DISPATCH(attn_backward_typed, rowptr, col, rowptr_t, col_t, t2csr, a, row_max, row_den, out, grad_out, pair, grad_v,
-                  grad_k, grad_q, grad_s_src, grad_s_dst, grad_att, gatt_part, b200mp_attn_gatt_rows(), n_rows, n_src, plan, plan_t,
-                  static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "attn_csr_backward", [&](auto tv, auto ti) {
+        return dispatch_attn_mode(mode, [&](auto m) {
+            return attn_backward_typed<decltype(tv), decltype(ti), m()>(
+                rowptr, col, rowptr_t, col_t, t2csr, a, row_max, row_den, out, grad_out, pair, grad_v, grad_k, grad_q,
+                grad_s_src, grad_s_dst, grad_att, gatt_part, b200mp_attn_gatt_rows(), n_rows, n_src, plan, plan_t,
+                static_cast<cudaStream_t>(stream));
+        });
+    });
 }

@@ -213,13 +213,8 @@ cg_reduce_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, CgArgs
         }
         if (is_chunk) {
 #pragma unroll
-            for (int o = 0; o < NACC; ++o) {
-                float* p = plan.partials + (static_cast<size_t>(item * NACC + o) * n_vec + vi) * EPV;
-#pragma unroll
-                for (int j = 0; j < EPV / 4; ++j)
-                    *reinterpret_cast<float4*>(p + 4 * j) =
-                        make_float4(acc[o][4 * j], acc[o][4 * j + 1], acc[o][4 * j + 2], acc[o][4 * j + 3]);
-            }
+            for (int o = 0; o < NACC; ++o)
+                store_partial<EPV>(plan.partials + (static_cast<size_t>(item * NACC + o) * n_vec + vi) * EPV, acc[o]);
             continue;
         }
         char* ob = static_cast<char*>(args.out) + row * R.out_ld * static_cast<int64_t>(sizeof(T));
@@ -335,19 +330,11 @@ int cg_typed(const void* rowptr_, const void* col_, CgArgs args, int64_t n_rows,
     const int64_t items = plan.n_chunks + n_rows;
     if (cg_vec_ok<T, MODE>(args, plan)) {
         const int n_vec = static_cast<int>(args.feat * sizeof(T) / 16);
-#define B200MP_L(G_)                                                                                             \
-    do {                                                                                                         \
-        const unsigned blocks = static_cast<unsigned>(ceil_div(items, 128 / G_));                                \
-        if (args.c) cg_reduce_kernel<T, I, MODE, G_, 4, true><<<blocks, 128, 0, stream>>>(rowptr, col, args, n_rows, n_vec, plan); \
-        else cg_reduce_kernel<T, I, MODE, G_, 4, false><<<blocks, 128, 0, stream>>>(rowptr, col, args, n_rows, n_vec, plan); \
-    } while (0)
-        if (n_vec <= 1) B200MP_L(1);
-        else if (n_vec <= 2) B200MP_L(2);
-        else if (n_vec <= 4) B200MP_L(4);
-        else if (n_vec <= 8) B200MP_L(8);
-        else if (n_vec <= 16) B200MP_L(16);
-        else B200MP_L(32);
-#undef B200MP_L
+        lane_group_shape<1>(n_vec, [&](auto G, auto) {
+            const unsigned blocks = static_cast<unsigned>(ceil_div(items, 128 / G()));
+            if (args.c) cg_reduce_kernel<T, I, MODE, G(), 4, true><<<blocks, 128, 0, stream>>>(rowptr, col, args, n_rows, n_vec, plan);
+            else cg_reduce_kernel<T, I, MODE, G(), 4, false><<<blocks, 128, 0, stream>>>(rowptr, col, args, n_rows, n_vec, plan);
+        });
     } else {
         cg_reduce_scalar_kernel<T, I, MODE><<<static_cast<unsigned>(ceil_div(items, 8)), 256, 0, stream>>>(
             rowptr, col, args, n_rows, plan);
@@ -360,58 +347,27 @@ int cg_typed(const void* rowptr_, const void* col_, CgArgs args, int64_t n_rows,
     return B200MP_OK;
 }
 
-template <typename T, typename I>
-int cg_fwd_typed(const void* rowptr, const void* col, CgArgs a, int64_t n, LongRowPlan p, cudaStream_t s) {
-    return cg_typed<T, I, kCgFwd>(rowptr, col, a, n, p, s);
-}
-template <typename T, typename I>
-int cg_dst_typed(const void* rowptr, const void* col, CgArgs a, int64_t n, LongRowPlan p, cudaStream_t s) {
-    return cg_typed<T, I, kCgDst>(rowptr, col, a, n, p, s);
-}
-template <typename T, typename I>
-int cg_src_typed(const void* rowptr, const void* col, CgArgs a, int64_t n, LongRowPlan p, cudaStream_t s) {
-    return cg_typed<T, I, kCgSrc>(rowptr, col, a, n, p, s);
-}
-
-inline LongRowPlan cg_plan(const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks,
-                           int64_t chunk, float* partials) {
-    return LongRowPlan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, partials,
-                       nullptr, 0, 0, nullptr, 0, nullptr};
-}
-
 }  // namespace b200mp
 
 using namespace b200mp;
-
-#define DISPATCH_T_I(FN, ...)                                                                                   \
-    do {                                                                                                        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) return FN<float, int32_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) return FN<float, int64_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) return FN<__nv_bfloat16, int32_t>(__VA_ARGS__); \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) return FN<__nv_bfloat16, int64_t>(__VA_ARGS__); \
-        set_error("unsupported dtype combination val=%d idx=%d", val_dtype, idx_dtype);                         \
-        return B200MP_ERR_UNSUPPORTED;                                                                          \
-    } while (0)
-
-#define B200MP_CHECK_CG()                                                                                       \
-    B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0);                                  \
-    B200MP_CHECK_ARG(ld_u >= 2 * feat && ld_v >= 2 * feat);                                                     \
-    B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);                                                        \
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && partials && chunk > 0))
 
 extern "C" int b200mp_cg_csr(const void* rowptr, const void* col, const void* perm, const void* u, const void* v,
                              const void* c, void* out, int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t feat,
                              int64_t ld_u, int64_t ld_v, int reduce, const int64_t* long_rows,
                              const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks, int64_t chunk,
                              float* partials, int idx_dtype, int val_dtype, void* stream) {
-    B200MP_CHECK_CG();
+    B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0);
+    B200MP_CHECK_ARG(ld_u >= 2 * feat && ld_v >= 2 * feat);
     B200MP_CHECK_ARG(reduce == B200MP_SUM || reduce == B200MP_MEAN);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && u && out);
     B200MP_CHECK_ARG(n_edges == 0 || (col && v));
     const CgArgs a{u, v, c, perm, nullptr, nullptr, out, nullptr, feat, ld_u, ld_v, reduce == B200MP_MEAN};
-    DISPATCH_T_I(cg_fwd_typed, rowptr, col, a, n_rows, cg_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials),
-                 static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "cg_csr", [&](auto tv, auto ti) {
+        return cg_typed<decltype(tv), decltype(ti), kCgFwd>(rowptr, col, a, n_rows, plan, static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_cg_backward_dst(const void* rowptr, const void* col, const void* perm, const void* u,
@@ -420,15 +376,19 @@ extern "C" int b200mp_cg_backward_dst(const void* rowptr, const void* col, const
                                       int64_t ld_v, int reduce, const int64_t* long_rows, const int64_t* chunk_ptr,
                                       int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials,
                                       int idx_dtype, int val_dtype, void* stream) {
-    B200MP_CHECK_CG();
+    B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0);
+    B200MP_CHECK_ARG(ld_u >= 2 * feat && ld_v >= 2 * feat);
     B200MP_CHECK_ARG(reduce == B200MP_SUM || reduce == B200MP_MEAN);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && u && grad_out && grad_u);
     B200MP_CHECK_ARG(n_edges == 0 || (col && v));
     B200MP_CHECK_ARG(grad_c == nullptr || c);
     const CgArgs a{u, v, c, perm, grad_out, nullptr, grad_u, grad_c, feat, ld_u, ld_v, reduce == B200MP_MEAN};
-    DISPATCH_T_I(cg_dst_typed, rowptr, col, a, n_rows, cg_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials),
-                 static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "cg_backward_dst", [&](auto tv, auto ti) {
+        return cg_typed<decltype(tv), decltype(ti), kCgDst>(rowptr, col, a, n_rows, plan, static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_cg_backward_src(const void* rowptr_t, const void* col_t, const void* perm_t, const float* val_t,
@@ -438,11 +398,16 @@ extern "C" int b200mp_cg_backward_src(const void* rowptr_t, const void* col_t, c
                                       int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials,
                                       int idx_dtype, int val_dtype, void* stream) {
     const int64_t n_rows = n_src, n_cols = n_dst;
-    B200MP_CHECK_CG();
+    B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0);
+    B200MP_CHECK_ARG(ld_u >= 2 * feat && ld_v >= 2 * feat);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_src == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr_t && v && grad_v);
     B200MP_CHECK_ARG(n_edges == 0 || (col_t && u && grad_out && (c == nullptr || perm_t)));
     const CgArgs a{u, v, c, perm_t, grad_out, val_t, grad_v, nullptr, feat, ld_u, ld_v, false};
-    DISPATCH_T_I(cg_src_typed, rowptr_t, col_t, a, n_src, cg_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials),
-                 static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "cg_backward_src", [&](auto tv, auto ti) {
+        return cg_typed<decltype(tv), decltype(ti), kCgSrc>(rowptr_t, col_t, a, n_src, plan,
+                                                          static_cast<cudaStream_t>(stream));
+    });
 }

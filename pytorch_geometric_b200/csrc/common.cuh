@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 #include <cstdio>
+#include <type_traits>
 
 #include "../../include/b200mp.h"
 
@@ -47,6 +48,40 @@ inline int num_sms() {
 }
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// Calls fn(T{}, I{}) for the supported (value dtype, index dtype) pairs: fp32 or bf16 values, int32 or int64 indices.
+template <typename F>
+int dispatch_val_idx(int val_dtype, int idx_dtype, const char* what, F&& fn) {
+    if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) return fn(float{}, int32_t{});
+    if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) return fn(float{}, int64_t{});
+    if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) return fn(__nv_bfloat16{}, int32_t{});
+    if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) return fn(__nv_bfloat16{}, int64_t{});
+    set_error("%s: unsupported dtype combination val=%d idx=%d", what, val_dtype, idx_dtype);
+    return B200MP_ERR_UNSUPPORTED;
+}
+
+// Lane-group shape of a row of n_vec 16-byte vectors: G = the smallest power of two >= n_vec, capped at a warp, and
+// VPL = vectors per lane, up to MAX_VPL (wider rows are walked by the kernel's own vbase loop).  Calls
+// launch(integral_constant<int, G>, integral_constant<int, VPL>).
+template <int MAX_VPL, typename F>
+void lane_group_shape(int n_vec, F&& launch) {
+    static_assert(MAX_VPL == 1 || MAX_VPL == 2 || MAX_VPL == 4, "VPL is 1, 2 or 4");
+    using std::integral_constant;
+    if (n_vec <= 1) launch(integral_constant<int, 1>{}, integral_constant<int, 1>{});
+    else if (n_vec <= 2) launch(integral_constant<int, 2>{}, integral_constant<int, 1>{});
+    else if (n_vec <= 4) launch(integral_constant<int, 4>{}, integral_constant<int, 1>{});
+    else if (n_vec <= 8) launch(integral_constant<int, 8>{}, integral_constant<int, 1>{});
+    else if (n_vec <= 16) launch(integral_constant<int, 16>{}, integral_constant<int, 1>{});
+    else if constexpr (MAX_VPL == 1) launch(integral_constant<int, 32>{}, integral_constant<int, 1>{});
+    else if (n_vec <= 32) launch(integral_constant<int, 32>{}, integral_constant<int, 1>{});
+    else if constexpr (MAX_VPL == 2) launch(integral_constant<int, 32>{}, integral_constant<int, 2>{});
+    else if (n_vec <= 64) launch(integral_constant<int, 32>{}, integral_constant<int, 2>{});
+    else launch(integral_constant<int, 32>{}, integral_constant<int, 4>{});
+}
+
+// Independent edges in flight per lane for VPL vectors per lane: about 4 sixteen-byte row loads.
+template <int VPL>
+constexpr int unroll_for_vpl() { return VPL >= 4 ? 1 : 4 / VPL; }
 
 // ---------------------------------------------------------------- 128-bit vector helpers
 struct __align__(16) Vec16 {
@@ -132,6 +167,20 @@ struct ElemTraits<__nv_bfloat16> {
     __device__ static __forceinline__ float to_float(__nv_bfloat16 x) { return __bfloat162float(x); }
     __device__ static __forceinline__ __nv_bfloat16 from_float(float x) { return __float2bfloat16_rn(x); }
 };
+
+// v rounded to the storage dtype T and back (a no-op for fp32): where the reference materialises a T tensor.
+template <typename T>
+__device__ __forceinline__ float round_to(float v) {
+    return ElemTraits<T>::to_float(ElemTraits<T>::from_float(v));
+}
+
+// A chunk's fp32 partial of one 16-byte vector (EPV elements) as EPV / 4 float4 stores.
+template <int EPV>
+__device__ __forceinline__ void store_partial(float* p, const float (&acc)[EPV]) {
+#pragma unroll
+    for (int q = 0; q < EPV / 4; ++q)
+        *reinterpret_cast<float4*>(p + 4 * q) = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
+}
 
 // ---------------------------------------------------------------- reductions
 // ATen amax/amin propagate NaN; fmaxf/fminf do not, so spell the comparison out.

@@ -51,6 +51,18 @@ struct LongRowPlan {
     const void* relu_mask;
 };
 
+// The plan of a C-ABI call from its six long-row arguments (include/b200mp.h): counts are non-negative, and long rows
+// need their row list, chunk offsets and a positive chunk, plus fp32 partials when `needs_partials` (sweeps that only
+// split rows write none).  Without long rows n_chunks is ignored.  The optional fields stay zero.
+inline int make_plan(LongRowPlan& plan, const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows,
+                     int64_t n_chunks, int64_t chunk, float* partials, bool needs_partials) {
+    B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);
+    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && chunk > 0 && (partials || !needs_partials)));
+    plan = LongRowPlan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, partials,
+                       nullptr, 0, 0, nullptr, 0, nullptr};
+    return B200MP_OK;
+}
+
 // Base address of source row c for the three addressing modes (plain, [local | halo], peer table).
 __device__ __forceinline__ const char* row_base(const LongRowPlan& plan, const char* xb, const char* xb2, int64_t split,
                                                 size_t row_bytes, int64_t c) {
@@ -212,15 +224,8 @@ csr_reduce_kernel(const I* __restrict__ rowptr, const I* __restrict__ col,
         if (is_chunk) {
             float* pbase = plan.partials + static_cast<size_t>(item) * n_vec * EPV;
 #pragma unroll
-            for (int k = 0; k < VPL; ++k) {
-                if (!vvalid[k]) continue;
-                float* p = pbase + static_cast<size_t>(vbase + lig + k * G) * EPV;
-#pragma unroll
-                for (int q = 0; q < EPV / 4; ++q) {
-                    float4 v = make_float4(acc[k][4 * q], acc[k][4 * q + 1], acc[k][4 * q + 2], acc[k][4 * q + 3]);
-                    *reinterpret_cast<float4*>(p + 4 * q) = v;
-                }
-            }
+            for (int k = 0; k < VPL; ++k)
+                if (vvalid[k]) store_partial<EPV>(pbase + static_cast<size_t>(vbase + lig + k * G) * EPV, acc[k]);
         } else {
             const int64_t deg = end - begin;
             char* ob = reinterpret_cast<char*>(out) + static_cast<size_t>(row) * row_bytes;
@@ -348,9 +353,8 @@ inline void launch_vec(const I* rowptr, const I* col, const float* val, const T*
     }
     // Default: occupancy over per-lane memory parallelism -- 4 sixteen-byte row loads in flight per lane, 128-thread CTAs,
     // registers capped at 40 (fp32) / 64 (bf16: twice the accumulators) => 48 / 32 warps per SM.
-    constexpr int kUnr = VPL >= 4 ? 1 : 4 / VPL;
-    if (sizeof(T) == 4) B200MP_LAUNCH_TUNED(kUnr, 128, 12);
-    else B200MP_LAUNCH_TUNED(kUnr, 128, 8);
+    if (sizeof(T) == 4) B200MP_LAUNCH_TUNED(unroll_for_vpl<VPL>(), 128, 12);
+    else B200MP_LAUNCH_TUNED(unroll_for_vpl<VPL>(), 128, 8);
 #undef B200MP_LAUNCH_TUNED
 }
 
@@ -365,17 +369,10 @@ int csr_reduce_dispatch(const I* rowptr, const I* col, const float* val, const T
                         aligned16(plan.relu_mask) && (plan.n_chunks == 0 || aligned16(plan.partials));
     if (vec_ok) {
         const int n_vec = static_cast<int>(row_bytes / 16);
-#define B200MP_LV(G_, V_) \
-    launch_vec<T, I, RED, GATHER, G_, V_>(rowptr, col, val, x, out, n_rows, n_vec, is_mean, inf_to_zero, plan, bias, stream)
-        if (n_vec <= 1) B200MP_LV(1, 1);
-        else if (n_vec <= 2) B200MP_LV(2, 1);
-        else if (n_vec <= 4) B200MP_LV(4, 1);
-        else if (n_vec <= 8) B200MP_LV(8, 1);
-        else if (n_vec <= 16) B200MP_LV(16, 1);
-        else if (n_vec <= 32) B200MP_LV(32, 1);
-        else if (n_vec <= 64) B200MP_LV(32, 2);
-        else B200MP_LV(32, 4);
-#undef B200MP_LV
+        lane_group_shape<4>(n_vec, [&](auto G, auto VPL) {
+            launch_vec<T, I, RED, GATHER, G(), VPL()>(rowptr, col, val, x, out, n_rows, n_vec, is_mean, inf_to_zero,
+                                                      plan, bias, stream);
+        });
     } else {
         int g = 1;
         while (g < 32 && g < feat) g <<= 1;

@@ -120,14 +120,8 @@ csr_tma_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, const fl
     auto flush_partial = [&](int64_t chunk_item) {
         float* pbase = plan.partials + static_cast<size_t>(chunk_item) * n_vec * EPV;
 #pragma unroll
-        for (int k = 0; k < VPL; ++k) {
-            if (!vvalid[k]) continue;
-            float* p = pbase + static_cast<size_t>(lane + k * 32) * EPV;
-#pragma unroll
-            for (int q = 0; q < EPV / 4; ++q)
-                *reinterpret_cast<float4*>(p + 4 * q) =
-                    make_float4(acc[k][4 * q], acc[k][4 * q + 1], acc[k][4 * q + 2], acc[k][4 * q + 3]);
-        }
+        for (int k = 0; k < VPL; ++k)
+            if (vvalid[k]) store_partial<EPV>(pbase + static_cast<size_t>(lane + k * 32) * EPV, acc[k]);
     };
 
     // Streams the edge range [e_begin, e_end).  Row bookkeeping: rows [row_lo, row_hi) of the unit

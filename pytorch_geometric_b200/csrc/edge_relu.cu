@@ -21,11 +21,6 @@
 
 namespace b200mp {
 
-template <typename T>
-__device__ __forceinline__ float round_to(float v) {
-    return ElemTraits<T>::to_float(ElemTraits<T>::from_float(v));
-}
-
 // Byte offset and bit shift of 16-byte vector v's first feature inside an edge's mask row.
 template <typename T>
 __device__ __forceinline__ int mask_byte(int v) { return ElemTraits<T>::kPerVec == 8 ? v : (v >> 1); }
@@ -50,10 +45,7 @@ template <typename T, int EPV>
 __device__ __forceinline__ void store_acc(const float (&acc)[EPV], bool is_chunk, int64_t item, int64_t row, int v,
                                           int n_vec, int64_t deg, bool is_mean, const LongRowPlan& plan, T* out) {
     if (is_chunk) {
-        float* p = plan.partials + (static_cast<size_t>(item) * n_vec + v) * EPV;
-#pragma unroll
-        for (int q = 0; q < EPV / 4; ++q)
-            *reinterpret_cast<float4*>(p + 4 * q) = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
+        store_partial<EPV>(plan.partials + (static_cast<size_t>(item) * n_vec + v) * EPV, acc);
     } else {
         float f[EPV];
 #pragma unroll
@@ -339,22 +331,6 @@ edge_relu_grad_edge_scalar_kernel(const I* __restrict__ rowptr, const I* __restr
 }
 
 // ---------------------------------------------------------------- host-side dispatch
-// The lane-group width / vectors-per-lane ladder of csr_reduce_dispatch; UNR edges in flight per lane.
-#define B200MP_EDGE_RELU_LADDER(LAUNCH)              \
-    do {                                             \
-        if (n_vec <= 1) LAUNCH(1, 1);                \
-        else if (n_vec <= 2) LAUNCH(2, 1);           \
-        else if (n_vec <= 4) LAUNCH(4, 1);           \
-        else if (n_vec <= 8) LAUNCH(8, 1);           \
-        else if (n_vec <= 16) LAUNCH(16, 1);         \
-        else if (n_vec <= 32) LAUNCH(32, 1);         \
-        else if (n_vec <= 64) LAUNCH(32, 2);         \
-        else LAUNCH(32, 4);                          \
-    } while (0)
-
-template <int VPL>
-constexpr int edge_relu_unroll() { return VPL >= 4 ? 1 : 4 / VPL; }
-
 inline bool edge_relu_vec_ok(int64_t feat, size_t elem, const void* p0, const void* p1, const void* p2,
                              const LongRowPlan& plan) {
     return (feat * elem) % 16 == 0 && aligned16(p0) && aligned16(p1) && aligned16(p2) &&
@@ -374,12 +350,11 @@ int edge_relu_forward_typed(const void* rowptr_, const void* col_, const void* p
     const int64_t items = plan.n_chunks + n_rows;
     if (edge_relu_vec_ok(feat, sizeof(T), x, a, out, plan)) {
         const int n_vec = static_cast<int>(feat * sizeof(T) / 16);
-#define B200MP_L(G_, V_)                                                                                         \
-    edge_relu_reduce_kernel<T, I, G_, V_, edge_relu_unroll<V_>()>                                                \
-        <<<static_cast<unsigned>(ceil_div(items, 128 / G_)), 128, 0, stream>>>(rowptr, col, perm, x, a, out, mask, \
-                                                                                n_rows, n_vec, mask_bytes, is_mean, plan)
-        B200MP_EDGE_RELU_LADDER(B200MP_L);
-#undef B200MP_L
+        lane_group_shape<4>(n_vec, [&](auto G, auto VPL) {
+            edge_relu_reduce_kernel<T, I, G(), VPL(), unroll_for_vpl<VPL()>()>
+                <<<static_cast<unsigned>(ceil_div(items, 128 / G())), 128, 0, stream>>>(
+                    rowptr, col, perm, x, a, out, mask, n_rows, n_vec, mask_bytes, is_mean, plan);
+        });
     } else {
         edge_relu_reduce_scalar_kernel<T, I><<<static_cast<unsigned>(ceil_div(items, 8)), 256, 0, stream>>>(
             rowptr, col, perm, x, a, out, mask, n_rows, feat, mask_bytes, is_mean, plan);
@@ -405,12 +380,11 @@ int edge_relu_grad_x_typed(const void* rowptr_t_, const void* col_t_, const void
     const int64_t items = plan.n_chunks + n_src;
     if (edge_relu_vec_ok(feat, sizeof(T), g, grad_x, nullptr, plan)) {
         const int n_vec = static_cast<int>(feat * sizeof(T) / 16);
-#define B200MP_L(G_, V_)                                                                                          \
-    edge_relu_grad_x_kernel<T, I, G_, V_, edge_relu_unroll<V_>()>                                                 \
-        <<<static_cast<unsigned>(ceil_div(items, 128 / G_)), 128, 0, stream>>>(rowptr_t, col_t, t2csr, val_t, g, mask, \
-                                                                                grad_x, n_src, n_vec, mask_bytes, plan)
-        B200MP_EDGE_RELU_LADDER(B200MP_L);
-#undef B200MP_L
+        lane_group_shape<4>(n_vec, [&](auto G, auto VPL) {
+            edge_relu_grad_x_kernel<T, I, G(), VPL(), unroll_for_vpl<VPL()>()>
+                <<<static_cast<unsigned>(ceil_div(items, 128 / G())), 128, 0, stream>>>(
+                    rowptr_t, col_t, t2csr, val_t, g, mask, grad_x, n_src, n_vec, mask_bytes, plan);
+        });
     } else {
         edge_relu_grad_x_scalar_kernel<T, I><<<static_cast<unsigned>(ceil_div(items, 8)), 256, 0, stream>>>(
             rowptr_t, col_t, t2csr, val_t, g, mask, grad_x, n_src, feat, mask_bytes, plan);
@@ -435,11 +409,11 @@ int edge_relu_grad_edge_typed(const void* rowptr_, const void* perm_, const void
     const int64_t items = plan.n_chunks + n_rows;
     if (edge_relu_vec_ok(feat, sizeof(T), g, grad_a, nullptr, plan)) {
         const int n_vec = static_cast<int>(feat * sizeof(T) / 16);
-#define B200MP_L(G_, V_)                                                                                           \
-    edge_relu_grad_edge_kernel<T, I, G_, V_><<<static_cast<unsigned>(ceil_div(items, 128 / G_)), 128, 0, stream>>>( \
-        rowptr, perm, g, mask, grad_a, n_rows, n_vec, mask_bytes, is_mean, plan)
-        B200MP_EDGE_RELU_LADDER(B200MP_L);
-#undef B200MP_L
+        lane_group_shape<4>(n_vec, [&](auto G, auto VPL) {
+            edge_relu_grad_edge_kernel<T, I, G(), VPL()><<<static_cast<unsigned>(ceil_div(items, 128 / G())), 128, 0,
+                                                           stream>>>(rowptr, perm, g, mask, grad_a, n_rows, n_vec,
+                                                                     mask_bytes, is_mean, plan);
+        });
     } else {
         edge_relu_grad_edge_scalar_kernel<T, I><<<static_cast<unsigned>(ceil_div(items, 8)), 256, 0, stream>>>(
             rowptr, perm, g, mask, grad_a, n_rows, feat, mask_bytes, is_mean, plan);
@@ -448,31 +422,9 @@ int edge_relu_grad_edge_typed(const void* rowptr_, const void* perm_, const void
     return B200MP_OK;
 }
 
-#undef B200MP_EDGE_RELU_LADDER
-
-inline LongRowPlan edge_relu_plan(const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows,
-                                  int64_t n_chunks, int64_t chunk, float* partials) {
-    return LongRowPlan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, partials,
-                       nullptr, 0, 0, nullptr, 0, nullptr};
-}
-
 }  // namespace b200mp
 
 using namespace b200mp;
-
-#define DISPATCH_T_I(FN, ...)                                                                                   \
-    do {                                                                                                        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) return FN<float, int32_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) return FN<float, int64_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) return FN<__nv_bfloat16, int32_t>(__VA_ARGS__); \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) return FN<__nv_bfloat16, int64_t>(__VA_ARGS__); \
-        set_error("unsupported dtype combination val=%d idx=%d", val_dtype, idx_dtype);                         \
-        return B200MP_ERR_UNSUPPORTED;                                                                          \
-    } while (0)
-
-#define B200MP_CHECK_PLAN()                                                                                     \
-    B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);                                                        \
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && partials && chunk > 0))
 
 extern "C" int b200mp_edge_relu_csr(const void* rowptr, const void* col, const void* perm, const void* x,
                                     const void* edge_rows, void* out, void* mask, int64_t n_rows, int64_t n_cols,
@@ -481,13 +433,16 @@ extern "C" int b200mp_edge_relu_csr(const void* rowptr, const void* col, const v
                                     float* partials, int idx_dtype, int val_dtype, void* stream) {
     B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0);
     B200MP_CHECK_ARG(reduce == B200MP_SUM || reduce == B200MP_MEAN);
-    B200MP_CHECK_PLAN();
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && out);
     B200MP_CHECK_ARG(n_edges == 0 || (col && x && edge_rows));
-    const LongRowPlan plan = edge_relu_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials);
-    DISPATCH_T_I(edge_relu_forward_typed, rowptr, col, perm, x, edge_rows, out, static_cast<uint8_t*>(mask), n_rows,
-                 feat, (feat + 7) / 8, reduce == B200MP_MEAN, plan, static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "edge_relu_csr", [&](auto tv, auto ti) {
+        return edge_relu_forward_typed<decltype(tv), decltype(ti)>(
+            rowptr, col, perm, x, edge_rows, out, static_cast<uint8_t*>(mask), n_rows, feat, (feat + 7) / 8,
+            reduce == B200MP_MEAN, plan, static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_edge_relu_backward_x(const void* rowptr_t, const void* col_t, const void* t2csr,
@@ -496,12 +451,15 @@ extern "C" int b200mp_edge_relu_backward_x(const void* rowptr_t, const void* col
                                            const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks,
                                            int64_t chunk, float* partials, int idx_dtype, int val_dtype, void* stream) {
     B200MP_CHECK_ARG(n_src >= 0 && feat >= 0);
-    B200MP_CHECK_PLAN();
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_src == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr_t && grad_x);
-    const LongRowPlan plan = edge_relu_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials);
-    DISPATCH_T_I(edge_relu_grad_x_typed, rowptr_t, col_t, t2csr, val_t, grad_out, static_cast<const uint8_t*>(mask),
-                 grad_x, n_src, feat, (feat + 7) / 8, plan, static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "edge_relu_backward_x", [&](auto tv, auto ti) {
+        return edge_relu_grad_x_typed<decltype(tv), decltype(ti)>(rowptr_t, col_t, t2csr, val_t, grad_out,
+                                                                static_cast<const uint8_t*>(mask), grad_x, n_src, feat,
+                                                                (feat + 7) / 8, plan, static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_edge_relu_backward_edge(const void* rowptr, const void* perm, const void* grad_out,
@@ -511,11 +469,14 @@ extern "C" int b200mp_edge_relu_backward_edge(const void* rowptr, const void* pe
                                               int val_dtype, void* stream) {
     B200MP_CHECK_ARG(n_rows >= 0 && feat >= 0);
     B200MP_CHECK_ARG(reduce == B200MP_SUM || reduce == B200MP_MEAN);
-    B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && chunk > 0));
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, nullptr, false)) return rc;
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && grad_out && grad_edge_rows);
-    const LongRowPlan plan = edge_relu_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, nullptr);
-    DISPATCH_T_I(edge_relu_grad_edge_typed, rowptr, perm, grad_out, static_cast<const uint8_t*>(mask), grad_edge_rows,
-                 n_rows, feat, (feat + 7) / 8, reduce == B200MP_MEAN, plan, static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "edge_relu_backward_edge", [&](auto tv, auto ti) {
+        return edge_relu_grad_edge_typed<decltype(tv), decltype(ti)>(rowptr, perm, grad_out,
+                                                                   static_cast<const uint8_t*>(mask), grad_edge_rows,
+                                                                   n_rows, feat, (feat + 7) / 8, reduce == B200MP_MEAN,
+                                                                   plan, static_cast<cudaStream_t>(stream));
+    });
 }

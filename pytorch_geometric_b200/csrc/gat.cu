@@ -306,19 +306,11 @@ int gat_fwd_typed(const void* rowptr_, const void* col_, const void* dst_of_edge
     if (vec_ok) {
         const int n_vec = static_cast<int>(row_bytes / 16);
         const int64_t items = plan.n_chunks + n_rows;
-#define GAT_LV(G_, V_)                                                                                      \
-    gat_fwd_vec_kernel<T, I, G_, V_><<<static_cast<unsigned>(ceil_div(items, kGatT / G_)), kGatT, 0, s>>>(    \
-        rowptr, col, xh, a_src, a_dst, out, row_max, row_den, n_rows, static_cast<int>(heads),              \
-        static_cast<int>(chan), n_vec, slope, plan, part_ms)
-        if (n_vec <= 1) GAT_LV(1, 1);
-        else if (n_vec <= 2) GAT_LV(2, 1);
-        else if (n_vec <= 4) GAT_LV(4, 1);
-        else if (n_vec <= 8) GAT_LV(8, 1);
-        else if (n_vec <= 16) GAT_LV(16, 1);
-        else if (n_vec <= 32) GAT_LV(32, 1);
-        else if (n_vec <= 64) GAT_LV(32, 2);
-        else GAT_LV(32, 4);
-#undef GAT_LV
+        lane_group_shape<4>(n_vec, [&](auto G, auto VPL) {
+            gat_fwd_vec_kernel<T, I, G(), VPL()><<<static_cast<unsigned>(ceil_div(items, kGatT / G())), kGatT, 0, s>>>(
+                rowptr, col, xh, a_src, a_dst, out, row_max, row_den, n_rows, static_cast<int>(heads),
+                static_cast<int>(chan), n_vec, slope, plan, part_ms);
+        });
         B200MP_LAUNCH_CHECK();
         if (plan.n_long > 0) {
             gat_combine_kernel<T><<<static_cast<unsigned>(plan.n_long), 256, 0, s>>>(out, row_max, row_den, static_cast<int>(heads),
@@ -375,16 +367,6 @@ int gat_bwd_typed(const void* rowptr, const void* col, const void* dst_of_edge, 
 
 using namespace b200mp;
 
-#define GAT_DISPATCH(FN, ...)                                                                                   \
-    do {                                                                                                        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) return FN<float, int32_t>(__VA_ARGS__);         \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) return FN<float, int64_t>(__VA_ARGS__);         \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) return FN<__nv_bfloat16, int32_t>(__VA_ARGS__); \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) return FN<__nv_bfloat16, int64_t>(__VA_ARGS__); \
-        set_error("gat: unsupported dtype combination val=%d idx=%d", val_dtype, idx_dtype);                    \
-        return B200MP_ERR_UNSUPPORTED;                                                                          \
-    } while (0)
-
 extern "C" int b200mp_gat_fused_csr(const void* rowptr, const void* col, const void* dst_of_edge, const void* xh,
                                     const float* a_src, const float* a_dst, void* out, float* row_max, float* row_den,
                                     float* alpha_out, int64_t n_rows, int64_t n_edges, int64_t heads, int64_t chan,
@@ -392,13 +374,17 @@ extern "C" int b200mp_gat_fused_csr(const void* rowptr, const void* col, const v
                                     int64_t n_chunks, int64_t chunk, float* part_acc, float* part_ms, int idx_dtype,
                                     int val_dtype, void* stream) {
     B200MP_CHECK_ARG(n_rows >= 0 && n_edges >= 0 && heads > 0 && chan > 0);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, part_acc, true)) return rc;
+    B200MP_CHECK_ARG(n_long_rows == 0 || part_ms);
     if (n_rows == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && a_dst && out && row_max && row_den);
     B200MP_CHECK_ARG(!alpha_out || dst_of_edge);
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && part_acc && part_ms && chunk > 0));
-    LongRowPlan plan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, part_acc};
-    GAT_DISPATCH(gat_fwd_typed, rowptr, col, dst_of_edge, xh, a_src, a_dst, out, row_max, row_den, alpha_out, n_rows,
-                 n_edges, heads, chan, slope, plan, part_ms, static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "gat_fused_csr", [&](auto tv, auto ti) {
+        return gat_fwd_typed<decltype(tv), decltype(ti)>(rowptr, col, dst_of_edge, xh, a_src, a_dst, out, row_max,
+                                                         row_den, alpha_out, n_rows, n_edges, heads, chan, slope, plan,
+                                                         part_ms, static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_gat_fused_csr_backward(const void* rowptr, const void* col, const void* dst_of_edge,
@@ -412,11 +398,14 @@ extern "C" int b200mp_gat_fused_csr_backward(const void* rowptr, const void* col
                                              int64_t chunk, float* partials, int idx_dtype, int val_dtype,
                                              void* stream) {
     B200MP_CHECK_ARG(n_rows >= 0 && n_src >= 0 && n_edges >= 0 && heads > 0 && chan > 0);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     B200MP_CHECK_ARG(rowptr && rowptr_t && grad_xh && grad_a_src && grad_a_dst && rowdot);
     B200MP_CHECK_ARG(n_edges == 0 || (dst_of_edge && grad_pre));
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && partials && chunk > 0));
-    LongRowPlan plan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, partials};
-    GAT_DISPATCH(gat_bwd_typed, rowptr, col, dst_of_edge, rowptr_t, col_t, t2csr, xh, a_src, a_dst, row_max, row_den, out,
-                 grad_out, grad_pre, rowdot, grad_xh, grad_a_src, grad_a_dst, n_rows, n_src, n_edges, heads, chan, slope,
-                 plan, static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "gat_fused_csr_backward", [&](auto tv, auto ti) {
+        return gat_bwd_typed<decltype(tv), decltype(ti)>(rowptr, col, dst_of_edge, rowptr_t, col_t, t2csr, xh, a_src,
+                                                         a_dst, row_max, row_den, out, grad_out, grad_pre, rowdot,
+                                                         grad_xh, grad_a_src, grad_a_dst, n_rows, n_src, n_edges, heads,
+                                                         chan, slope, plan, static_cast<cudaStream_t>(stream));
+    });
 }

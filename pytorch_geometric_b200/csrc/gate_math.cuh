@@ -5,12 +5,6 @@
 
 namespace b200mp {
 
-// v rounded to the storage dtype T and back (a no-op for fp32): where the reference materialises a T tensor.
-template <typename T>
-__device__ __forceinline__ float round_to(float v) {
-    return ElemTraits<T>::to_float(ElemTraits<T>::from_float(v));
-}
-
 // sigma(s) and sigma'(s) from t = exp(-|s|) by __expf (ex2.approx) and r = 1 / (1 + t) by __fdividef (rcp.approx): two
 // MUFU operations.  sigma = s >= 0 ? r : t * r and sigma' = t * r * r -- never sigma * (1 - sigma), which cancels at
 // large |s|.  s = +inf gives 1, 0; s = -inf gives 0, 0; NaN stays NaN (s >= 0 is false, t = NaN).

@@ -167,13 +167,8 @@ gated_reduce_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, Gat
             const int v = vbase + lig + k * G;
             if (is_chunk) {
 #pragma unroll
-                for (int o = 0; o < NACC; ++o) {
-                    float* p = plan.partials + (static_cast<size_t>(item * NACC + o) * n_vec + v) * EPV;
-#pragma unroll
-                    for (int j = 0; j < EPV / 4; ++j)
-                        *reinterpret_cast<float4*>(p + 4 * j) =
-                            make_float4(acc[o][k][4 * j], acc[o][k][4 * j + 1], acc[o][k][4 * j + 2], acc[o][k][4 * j + 3]);
-                }
+                for (int o = 0; o < NACC; ++o)
+                    store_partial<EPV>(plan.partials + (static_cast<size_t>(item * NACC + o) * n_vec + v) * EPV, acc[o][k]);
                 continue;
             }
             float mul[EPV];
@@ -253,22 +248,6 @@ gated_combine_kernel(const I* __restrict__ rowptr, GatedArgs args, LongRowPlan p
 }
 
 // ---------------------------------------------------------------- host-side dispatch
-// The lane-group width / vectors-per-lane ladder of csr_reduce_dispatch; UNR edges in flight per lane.
-#define B200MP_GATED_LADDER(LAUNCH)                  \
-    do {                                             \
-        if (n_vec <= 1) LAUNCH(1, 1);                \
-        else if (n_vec <= 2) LAUNCH(2, 1);           \
-        else if (n_vec <= 4) LAUNCH(4, 1);           \
-        else if (n_vec <= 8) LAUNCH(8, 1);           \
-        else if (n_vec <= 16) LAUNCH(16, 1);         \
-        else if (n_vec <= 32) LAUNCH(32, 1);         \
-        else if (n_vec <= 64) LAUNCH(32, 2);         \
-        else LAUNCH(32, 4);                          \
-    } while (0)
-
-template <int VPL>
-constexpr int gated_unroll() { return VPL >= 4 ? 1 : 4 / VPL; }
-
 template <typename T, int MODE>
 bool gated_vec_ok(const GatedArgs& a, const LongRowPlan& plan) {
     return (a.feat * sizeof(T)) % 16 == 0 && (a.ld * sizeof(T)) % 16 == 0 && aligned16(a.k) && aligned16(a.q) &&
@@ -284,11 +263,11 @@ int gated_typed(const void* rowptr_, const void* col_, GatedArgs args, int64_t n
     const int64_t items = plan.n_chunks + n_rows;
     if (gated_vec_ok<T, MODE>(args, plan)) {
         const int n_vec = static_cast<int>(args.feat * sizeof(T) / 16);
-#define B200MP_L(G_, V_)                                                                                      \
-    gated_reduce_kernel<T, I, MODE, G_, V_, gated_unroll<V_>()>                                               \
-        <<<static_cast<unsigned>(ceil_div(items, 128 / G_)), 128, 0, stream>>>(rowptr, col, args, n_rows, n_vec, plan)
-        B200MP_GATED_LADDER(B200MP_L);
-#undef B200MP_L
+        lane_group_shape<4>(n_vec, [&](auto G, auto VPL) {
+            gated_reduce_kernel<T, I, MODE, G(), VPL(), unroll_for_vpl<VPL()>()>
+                <<<static_cast<unsigned>(ceil_div(items, 128 / G())), 128, 0, stream>>>(rowptr, col, args, n_rows, n_vec,
+                                                                                       plan);
+        });
     } else {
         gated_reduce_scalar_kernel<T, I, MODE><<<static_cast<unsigned>(ceil_div(items, 8)), 256, 0, stream>>>(
             rowptr, col, args, n_rows, plan);
@@ -301,59 +280,27 @@ int gated_typed(const void* rowptr_, const void* col_, GatedArgs args, int64_t n
     return B200MP_OK;
 }
 
-#undef B200MP_GATED_LADDER
-
-template <typename T, typename I>
-int gated_fwd_typed(const void* rowptr, const void* col, GatedArgs a, int64_t n, LongRowPlan p, cudaStream_t s) {
-    return gated_typed<T, I, kGatedFwd>(rowptr, col, a, n, p, s);
-}
-template <typename T, typename I>
-int gated_dst_typed(const void* rowptr, const void* col, GatedArgs a, int64_t n, LongRowPlan p, cudaStream_t s) {
-    return gated_typed<T, I, kGatedDst>(rowptr, col, a, n, p, s);
-}
-template <typename T, typename I>
-int gated_src_typed(const void* rowptr, const void* col, GatedArgs a, int64_t n, LongRowPlan p, cudaStream_t s) {
-    return gated_typed<T, I, kGatedSrc>(rowptr, col, a, n, p, s);
-}
-
-inline LongRowPlan gated_plan(const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows,
-                              int64_t n_chunks, int64_t chunk, float* partials) {
-    return LongRowPlan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, partials,
-                       nullptr, 0, 0, nullptr, 0, nullptr};
-}
-
 }  // namespace b200mp
 
 using namespace b200mp;
-
-#define DISPATCH_T_I(FN, ...)                                                                                   \
-    do {                                                                                                        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) return FN<float, int32_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) return FN<float, int64_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) return FN<__nv_bfloat16, int32_t>(__VA_ARGS__); \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) return FN<__nv_bfloat16, int64_t>(__VA_ARGS__); \
-        set_error("unsupported dtype combination val=%d idx=%d", val_dtype, idx_dtype);                         \
-        return B200MP_ERR_UNSUPPORTED;                                                                          \
-    } while (0)
-
-#define B200MP_CHECK_GATED()                                                                                    \
-    B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0 && ld >= feat);                    \
-    B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);                                                        \
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && partials && chunk > 0))
 
 extern "C" int b200mp_gated_csr(const void* rowptr, const void* col, const void* k, const void* q, const void* v,
                                 void* out, int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t feat, int64_t ld,
                                 int reduce, const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows,
                                 int64_t n_chunks, int64_t chunk, float* partials, int idx_dtype, int val_dtype,
                                 void* stream) {
-    B200MP_CHECK_GATED();
+    B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0 && ld >= feat);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     B200MP_CHECK_ARG(reduce == B200MP_SUM || reduce == B200MP_MEAN);
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && k && out);
     B200MP_CHECK_ARG(n_edges == 0 || (col && q && v));
     const GatedArgs a{k, q, v, nullptr, nullptr, out, nullptr, feat, ld, reduce == B200MP_MEAN};
-    DISPATCH_T_I(gated_fwd_typed, rowptr, col, a, n_rows,
-                 gated_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials), static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "gated_csr", [&](auto tv, auto ti) {
+        return gated_typed<decltype(tv), decltype(ti), kGatedFwd>(rowptr, col, a, n_rows, plan,
+                                                                static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_gated_backward_dst(const void* rowptr, const void* col, const void* k, const void* q,
@@ -362,14 +309,18 @@ extern "C" int b200mp_gated_backward_dst(const void* rowptr, const void* col, co
                                          const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows,
                                          int64_t n_chunks, int64_t chunk, float* partials, int idx_dtype,
                                          int val_dtype, void* stream) {
-    B200MP_CHECK_GATED();
+    B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0 && ld >= feat);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     B200MP_CHECK_ARG(reduce == B200MP_SUM || reduce == B200MP_MEAN);
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && k && grad_out && grad_k);
     B200MP_CHECK_ARG(n_edges == 0 || (col && q && v));
     const GatedArgs a{k, q, v, grad_out, nullptr, grad_k, nullptr, feat, ld, reduce == B200MP_MEAN};
-    DISPATCH_T_I(gated_dst_typed, rowptr, col, a, n_rows,
-                 gated_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials), static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "gated_backward_dst", [&](auto tv, auto ti) {
+        return gated_typed<decltype(tv), decltype(ti), kGatedDst>(rowptr, col, a, n_rows, plan,
+                                                                static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_gated_backward_src(const void* rowptr_t, const void* col_t, const float* val_t, const void* k,
@@ -379,11 +330,15 @@ extern "C" int b200mp_gated_backward_src(const void* rowptr_t, const void* col_t
                                          int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials,
                                          int idx_dtype, int val_dtype, void* stream) {
     const int64_t n_rows = n_src, n_cols = n_dst;
-    B200MP_CHECK_GATED();
+    B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0 && ld >= feat);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_src == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr_t && q && v && grad_q && grad_v);
     B200MP_CHECK_ARG(n_edges == 0 || (col_t && k && grad_out));
     const GatedArgs a{k, q, v, grad_out, val_t, grad_v, grad_q, feat, ld, false};
-    DISPATCH_T_I(gated_src_typed, rowptr_t, col_t, a, n_src,
-                 gated_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials), static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "gated_backward_src", [&](auto tv, auto ti) {
+        return gated_typed<decltype(tv), decltype(ti), kGatedSrc>(rowptr_t, col_t, a, n_src, plan,
+                                                                static_cast<cudaStream_t>(stream));
+    });
 }

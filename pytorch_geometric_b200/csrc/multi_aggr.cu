@@ -845,16 +845,10 @@ void multi_launch_mode(const I* rowptr, const I* col, const T* x, const MultiOut
     // free as soon as ITS rows are done instead of after the longest row of four warps (power-law degrees); multi_tune 5 =
     // the 128-thread form, kept for A/B
     const int bt = get_option_multi_tune() == 5 ? 128 : 32;
-#define B200MP_MA(G_)                                                                                            \
-    multi_aggr_kernel<T, I, G_, GATHER, MODE><<<static_cast<unsigned>(ceil_div(items, bt / G_)), bt, 0, stream>>>( \
-        rowptr, col, x, outs, n_rows, n_vec, plan)
-    if (n_vec <= 1) B200MP_MA(1);
-    else if (n_vec <= 2) B200MP_MA(2);
-    else if (n_vec <= 4) B200MP_MA(4);
-    else if (n_vec <= 8) B200MP_MA(8);
-    else if (n_vec <= 16) B200MP_MA(16);
-    else B200MP_MA(32);
-#undef B200MP_MA
+    lane_group_shape<1>(n_vec, [&](auto G, auto) {
+        multi_aggr_kernel<T, I, G(), GATHER, MODE><<<static_cast<unsigned>(ceil_div(items, bt / G())), bt, 0, stream>>>(
+            rowptr, col, x, outs, n_rows, n_vec, plan);
+    });
 }
 
 template <typename T, typename I, bool GATHER>
@@ -922,16 +916,10 @@ int multi_typed(const void* rowptr, const void* col, const void* x, MultiOut out
 template <typename I>
 void multi_bwd_vec_launch(const I* ptr, const I* idx, const float* x, const MultiGrad& g, float* grad_x,
                           int64_t n_items, int n_vec, cudaStream_t stream) {
-#define B200MP_MB(G_)                                                                                        \
-    multi_aggr_backward_vec_kernel<I, G_><<<static_cast<unsigned>(ceil_div(n_items, 128 / G_)), 128, 0, stream>>>( \
-        ptr, idx, x, g, grad_x, n_items, n_vec)
-    if (n_vec <= 1) B200MP_MB(1);
-    else if (n_vec <= 2) B200MP_MB(2);
-    else if (n_vec <= 4) B200MP_MB(4);
-    else if (n_vec <= 8) B200MP_MB(8);
-    else if (n_vec <= 16) B200MP_MB(16);
-    else B200MP_MB(32);
-#undef B200MP_MB
+    lane_group_shape<1>(n_vec, [&](auto G, auto) {
+        multi_aggr_backward_vec_kernel<I, G()><<<static_cast<unsigned>(ceil_div(n_items, 128 / G())), 128, 0, stream>>>(
+            ptr, idx, x, g, grad_x, n_items, n_vec);
+    });
 }
 
 // Segment-mode backward (one destination per message, messages sorted by destination): a lane group walks kSegRun
@@ -999,15 +987,10 @@ template <typename I>
 void multi_bwd_segment_launch(const I* idx, const float* x, const MultiGrad& g, float* grad_x, int64_t n_msgs, int n_vec,
                               cudaStream_t stream) {
     const int64_t items = ceil_div(n_msgs, kSegRun);
-#define B200MP_MS(G_) \
-    multi_aggr_backward_segment_kernel<I, G_><<<static_cast<unsigned>(ceil_div(items, 128 / G_)), 128, 0, stream>>>(idx, x, g, grad_x, n_msgs, n_vec)
-    if (n_vec <= 1) B200MP_MS(1);
-    else if (n_vec <= 2) B200MP_MS(2);
-    else if (n_vec <= 4) B200MP_MS(4);
-    else if (n_vec <= 8) B200MP_MS(8);
-    else if (n_vec <= 16) B200MP_MS(16);
-    else B200MP_MS(32);
-#undef B200MP_MS
+    lane_group_shape<1>(n_vec, [&](auto G, auto) {
+        multi_aggr_backward_segment_kernel<I, G()><<<static_cast<unsigned>(ceil_div(items, 128 / G())), 128, 0, stream>>>(
+            idx, x, g, grad_x, n_msgs, n_vec);
+    });
 }
 
 template <typename T, typename I>
@@ -1058,16 +1041,6 @@ int multi_bwd_typed(const void* ptr, const void* idx, const void* x, MultiGrad g
 
 using namespace b200mp;
 
-#define DISPATCH_T_I(FN, ...)                                                        \
-    do {                                                                             \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) return FN<float, int32_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) return FN<float, int64_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) return FN<__nv_bfloat16, int32_t>(__VA_ARGS__); \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) return FN<__nv_bfloat16, int64_t>(__VA_ARGS__); \
-        set_error("unsupported dtype combination val=%d idx=%d", val_dtype, idx_dtype);                         \
-        return B200MP_ERR_UNSUPPORTED;                                                                          \
-    } while (0)
-
 extern "C" int b200mp_multi_aggr_mask_supported(int64_t feat, int val_dtype, int segment_mode) {
     return val_dtype == B200MP_F32 && !segment_mode && feat % 4 == 0 && feat > 64 && feat <= 256 && get_option_attn_staged();
 }
@@ -1079,17 +1052,18 @@ extern "C" int b200mp_multi_aggr_csr(const void* rowptr, const void* col, const 
                                      const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks,
                                      int64_t chunk, float* partials, int idx_dtype, int val_dtype, void* stream) {
     B200MP_CHECK_ARG(n_rows >= 0 && n_src >= 0 && feat >= 0);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && (x || n_src == 0));
-    B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && partials && chunk > 0));
     // the hit mask is a by-product of the tie-counting fp32 vector sweep in gather mode
     B200MP_CHECK_ARG(!hit_mask || (col && b200mp_multi_aggr_mask_supported(feat, val_dtype, 0) && (ties_min || ties_max)));
     MultiOut outs{{out_sum, out_mean, out_min, out_max, out_var, out_std, ties_min, ties_max}, count_self_zero != 0,
                   static_cast<uint8_t*>(hit_mask)};
-    LongRowPlan plan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, partials,
-                     nullptr, 0, 0, nullptr, 0};
-    DISPATCH_T_I(multi_typed, rowptr, col, x, outs, n_rows, feat, plan, static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "multi_aggr_csr", [&](auto tv, auto ti) {
+        return multi_typed<decltype(tv), decltype(ti)>(rowptr, col, x, outs, n_rows, feat, plan,
+                                                       static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_multi_aggr_backward(const void* ptr, const void* idx, const void* x, const float* term_a,
@@ -1108,8 +1082,10 @@ extern "C" int b200mp_multi_aggr_backward(const void* ptr, const void* idx, cons
     MultiGrad g{term_a, term_b, masked ? nullptr : out_min, g_min, masked ? nullptr : out_max, g_max,
                 masked ? static_cast<const uint8_t*>(hit_mask) : nullptr, masked ? t2csr : nullptr};
     B200MP_CHECK_ARG(masked || ((!g_min || out_min) && (!g_max || out_max)));
-    DISPATCH_T_I(multi_bwd_typed, ptr, idx, x, g, grad_x, n_items, feat, segment_mode,
-                 static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "multi_aggr_backward", [&](auto tv, auto ti) {
+        return multi_bwd_typed<decltype(tv), decltype(ti)>(ptr, idx, x, g, grad_x, n_items, feat, segment_mode,
+                                                           static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_multi_aggr_prepare_backward(const void* rowptr, const void* g_sum, const void* g_mean,
@@ -1130,5 +1106,8 @@ extern "C" int b200mp_multi_aggr_prepare_backward(const void* rowptr, const void
     MultiPrep p{g_sum, g_mean, g_var, g_std, g_min, g_max, mean, std, ties_min, ties_max,
                 (g_sum || g_mean || g_var || g_std) ? term_a : nullptr, (g_var || g_std) ? term_b : nullptr,
                 gmin_out, gmax_out};
-    DISPATCH_T_I(multi_prep_typed, rowptr, p, n_rows, feat, semi_grad, static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "multi_aggr_prepare_backward", [&](auto tv, auto ti) {
+        return multi_prep_typed<decltype(tv), decltype(ti)>(rowptr, p, n_rows, feat, semi_grad,
+                                                            static_cast<cudaStream_t>(stream));
+    });
 }

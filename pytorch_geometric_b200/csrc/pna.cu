@@ -40,11 +40,6 @@ struct PnaStats {                         // statistics of w, [n_rows, W]: sum /
     const float *ties_min, *ties_max;
 };
 
-template <typename T>
-__device__ __forceinline__ float pna_round(float v) {
-    return ElemTraits<T>::to_float(ElemTraits<T>::from_float(v));
-}
-
 // scaler factor (scaler.py:92-107) for a degree already rounded to the output dtype
 __device__ __forceinline__ float pna_factor(int s, float d, float lin, float lg) {
     switch (s) {
@@ -70,15 +65,15 @@ __device__ __forceinline__ void pna_aggregates(const PnaStats& st, size_t di, fl
     auto ld = [&](const void* p) { return p ? ElemTraits<S>::to_float(static_cast<const S*>(p)[di]) : 0.f; };
     sum_w = ld(st.sum);
     const float s = __fadd_rn(__fmul_rn(static_cast<float>(deg), u), sum_w);
-    agg[PA_SUM] = pna_round<T>(s);
-    agg[PA_MEAN] = pna_round<T>(__fdiv_rn(s, cnt));
-    agg[PA_MIN] = deg == 0 ? 0.f : pna_round<T>(__fadd_rn(u, ld(st.mn)));
-    agg[PA_MAX] = deg == 0 ? 0.f : pna_round<T>(__fadd_rn(u, ld(st.mx)));
+    agg[PA_SUM] = round_to<T>(s);
+    agg[PA_MEAN] = round_to<T>(__fdiv_rn(s, cnt));
+    agg[PA_MIN] = deg == 0 ? 0.f : round_to<T>(__fadd_rn(u, ld(st.mn)));
+    agg[PA_MAX] = deg == 0 ? 0.f : round_to<T>(__fadd_rn(u, ld(st.mx)));
     const float var = ld(st.var);
     float sd = __fsqrt_rn(var < 1e-5f ? 1e-5f : var);
     if (sd <= static_cast<float>(0.0031622776601683794)) sd = 0.f;            // math.sqrt(1e-5), basic.py:136
-    agg[PA_VAR] = pna_round<T>(var);
-    agg[PA_STD] = pna_round<T>(sd);
+    agg[PA_VAR] = round_to<T>(var);
+    agg[PA_STD] = round_to<T>(sd);
 }
 
 // agg[kind] without a dynamically indexed (local-memory) array
@@ -98,11 +93,11 @@ pna_epilogue_kernel(const I* __restrict__ rowptr, const T* __restrict__ x, const
     const int64_t row = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
     if (row >= n_rows) return;
     const int64_t deg = static_cast<int64_t>(rowptr[row + 1]) - static_cast<int64_t>(rowptr[row]);
-    const float d = pna_round<T>(static_cast<float>(deg));       // degree(..., dtype=out.dtype) on the CPU, scaler.py:82
+    const float d = round_to<T>(static_cast<float>(deg));       // degree(..., dtype=out.dtype) on the CPU, scaler.py:82
     const float lin = *sh.avg_lin, lg = *sh.avg_log;
     float fac[kPnaMaxScaler];
 #pragma unroll
-    for (int s = 0; s < kPnaMaxScaler; ++s) fac[s] = s < sh.n_scaler ? pna_round<T>(pna_factor(sh.scaler[s], d, lin, lg)) : 0.f;
+    for (int s = 0; s < kPnaMaxScaler; ++s) fac[s] = s < sh.n_scaler ? round_to<T>(pna_factor(sh.scaler[s], d, lin, lg)) : 0.f;
     const int64_t W = sh.towers * sh.feat, slots = 1 + static_cast<int64_t>(sh.n_aggr) * sh.n_scaler;
     T* orow = out + static_cast<size_t>(row) * W * slots;
     for (int64_t c = lane; c < W; c += 32) {
@@ -142,12 +137,12 @@ pna_prologue_kernel(const I* __restrict__ rowptr, const T* __restrict__ u, int64
     if (row >= n_rows) return;
     const int64_t deg = static_cast<int64_t>(rowptr[row + 1]) - static_cast<int64_t>(rowptr[row]);
     const float cnt = static_cast<float>(deg < 1 ? 1 : deg);
-    const float d = pna_round<T>(static_cast<float>(deg));
+    const float d = round_to<T>(static_cast<float>(deg));
     const float lin = *sh.avg_lin, lg = *sh.avg_log;
     float fac[kPnaMaxScaler], dlin[kPnaMaxScaler], dlog[kPnaMaxScaler];
 #pragma unroll
     for (int s = 0; s < kPnaMaxScaler; ++s) {
-        fac[s] = s < sh.n_scaler ? pna_round<T>(pna_factor(sh.scaler[s], d, lin, lg)) : 0.f;
+        fac[s] = s < sh.n_scaler ? round_to<T>(pna_factor(sh.scaler[s], d, lin, lg)) : 0.f;
         pna_factor_grad(s < sh.n_scaler ? sh.scaler[s] : PS_IDENTITY, fac[s], lin, lg, dlin[s], dlog[s]);
     }
     const int64_t W = sh.towers * sh.feat, slots = 1 + static_cast<int64_t>(sh.n_aggr) * sh.n_scaler;
@@ -252,7 +247,7 @@ __device__ __forceinline__ void ps_store(const PnaStatsOut& o, size_t di, const 
 // Linear would produce in that dtype, before the destination's shift)
 template <typename T>
 __device__ __forceinline__ float pna_w(const T* v, int64_t v_ld, const T* c, int64_t W, int64_t j, int64_t ce, int64_t cidx) {
-    return pna_round<T>(__fadd_rn(ElemTraits<T>::to_float(v[static_cast<size_t>(j) * v_ld + cidx]),
+    return round_to<T>(__fadd_rn(ElemTraits<T>::to_float(v[static_cast<size_t>(j) * v_ld + cidx]),
                                   ElemTraits<T>::to_float(c[static_cast<size_t>(ce) * W + cidx])));
 }
 
@@ -459,16 +454,6 @@ inline int pna_shape(PnaShape& sh, const int32_t* aggr_host, int n_aggr, const i
 
 using namespace b200mp;
 
-#define DISPATCH_T_I(FN, ...)                                                                                   \
-    do {                                                                                                        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) return FN<float, int32_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) return FN<float, int64_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) return FN<__nv_bfloat16, int32_t>(__VA_ARGS__); \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) return FN<__nv_bfloat16, int64_t>(__VA_ARGS__); \
-        set_error("unsupported dtype combination val=%d idx=%d", val_dtype, idx_dtype);                         \
-        return B200MP_ERR_UNSUPPORTED;                                                                          \
-    } while (0)
-
 extern "C" int b200mp_pna_epilogue(const void* rowptr, const void* x, const void* u, int64_t u_ld, const void* stat_sum,
                                    const void* stat_min, const void* stat_max, const void* stat_var,
                                    const int32_t* aggr_host, int n_aggr, const int32_t* scaler_host, int n_scaler,
@@ -482,8 +467,11 @@ extern "C" int b200mp_pna_epilogue(const void* rowptr, const void* x, const void
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && x && u && out);
     const PnaStats st{stat_sum, stat_min, stat_max, stat_var, nullptr, nullptr};
-    DISPATCH_T_I(pna_epilogue_typed, rowptr, x, u, u_ld, st, sh, out, n_rows, stats_dtype == B200MP_F32 && val_dtype != B200MP_F32,
-                 static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "pna_epilogue", [&](auto tv, auto ti) {
+        return pna_epilogue_typed<decltype(tv), decltype(ti)>(rowptr, x, u, u_ld, st, sh, out, n_rows,
+                                                              stats_dtype == B200MP_F32 && val_dtype != B200MP_F32,
+                                                              static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_pna_prologue(const void* rowptr, const void* grad_out, const void* u, int64_t u_ld,
@@ -504,8 +492,11 @@ extern "C" int b200mp_pna_prologue(const void* rowptr, const void* grad_out, con
     B200MP_CHECK_ARG(!gmax || (stat_max && ties_max));
     const PnaStats st{stat_sum, stat_min, stat_max, stat_var, ties_min, ties_max};
     const PnaBwd b{grad_out, term_a, term_b, gmin, gmax, grad_u, gu_ld, grad_x, avg_part};
-    DISPATCH_T_I(pna_prologue_typed, rowptr, u, u_ld, st, sh, b, n_rows, stats_dtype == B200MP_F32 && val_dtype != B200MP_F32,
-                 static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "pna_prologue", [&](auto tv, auto ti) {
+        return pna_prologue_typed<decltype(tv), decltype(ti)>(rowptr, u, u_ld, st, sh, b, n_rows,
+                                                              stats_dtype == B200MP_F32 && val_dtype != B200MP_F32,
+                                                              static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_pna_edge_stats(const void* rowptr, const void* col, const void* perm, const void* v, int64_t v_ld,
@@ -515,14 +506,15 @@ extern "C" int b200mp_pna_edge_stats(const void* rowptr, const void* col, const 
                                      int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials, int idx_dtype,
                                      int val_dtype, void* stream) {
     B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && width >= 0 && v_ld >= width);
-    B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && partials && chunk > 0));
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_rows == 0 || width == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && (n_edges == 0 || (col && v && c)));
     const PnaStatsOut so{stat_sum, stat_min, stat_max, stat_var, ties_min, ties_max};
-    const LongRowPlan plan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, partials,
-                           nullptr, 0, 0, nullptr, 0};
-    DISPATCH_T_I(pna_edge_stats_typed, rowptr, col, perm, v, v_ld, c, so, n_rows, width, plan, static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "pna_edge_stats", [&](auto tv, auto ti) {
+        return pna_edge_stats_typed<decltype(tv), decltype(ti)>(rowptr, col, perm, v, v_ld, c, so, n_rows, width, plan,
+                                                                static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_pna_edge_backward(const void* rowptr_t, const void* col_t, const void* perm_t, const void* v,
@@ -538,6 +530,8 @@ extern "C" int b200mp_pna_edge_backward(const void* rowptr_t, const void* col_t,
     B200MP_CHECK_ARG(n_edges == 0 || (col_t && perm_t && c));
     B200MP_CHECK_ARG((!gmin || stat_min) && (!gmax || stat_max));
     const PnaEdgeGrad g{term_a, term_b, stat_min, gmin, stat_max, gmax};
-    DISPATCH_T_I(pna_edge_backward_typed, rowptr_t, col_t, perm_t, v, v_ld, c, g, grad_v, gv_ld, grad_c, n_src, width,
-                 static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "pna_edge_backward", [&](auto tv, auto ti) {
+        return pna_edge_backward_typed<decltype(tv), decltype(ti)>(rowptr_t, col_t, perm_t, v, v_ld, c, g, grad_v, gv_ld,
+                                                                   grad_c, n_src, width, static_cast<cudaStream_t>(stream));
+    });
 }

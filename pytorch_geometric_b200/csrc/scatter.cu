@@ -222,11 +222,7 @@ extern "C" int b200mp_gather_rows(const void* x, const void* index, const float*
     B200MP_CHECK_ARG(n_out >= 0 && feat >= 0);
     if (n_out == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(x && index && out);
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) return gather_typed<float, int32_t>(x, index, scale, out, n_out, feat, s);
-    if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) return gather_typed<float, int64_t>(x, index, scale, out, n_out, feat, s);
-    if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) return gather_typed<__nv_bfloat16, int32_t>(x, index, scale, out, n_out, feat, s);
-    if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) return gather_typed<__nv_bfloat16, int64_t>(x, index, scale, out, n_out, feat, s);
-    set_error("gather_rows: unsupported dtype combination");
-    return B200MP_ERR_UNSUPPORTED;
+    return dispatch_val_idx(val_dtype, idx_dtype, "gather_rows", [&](auto tv, auto ti) {
+        return gather_typed<decltype(tv), decltype(ti)>(x, index, scale, out, n_out, feat, static_cast<cudaStream_t>(stream));
+    });
 }

@@ -3,33 +3,21 @@
 
 using namespace b200mp;
 
-namespace b200mp {
-template <typename T, typename I>
-int segment_typed(const void* ptr, const void* src, void* out, int64_t n_rows, int64_t feat, int reduce,
-                  LongRowPlan plan, cudaStream_t stream) {
-    return csr_reduce_auto<T, I, false>(static_cast<const I*>(ptr), static_cast<const I*>(nullptr), nullptr,
-                                         static_cast<const T*>(src), static_cast<T*>(out), n_rows, feat,
-                                         reduce, true, plan, nullptr, stream);
-}
-}  // namespace b200mp
-
 extern "C" int b200mp_segment_csr(const void* ptr, const void* src, void* out, int64_t n_rows,
                                   int64_t n_src, int64_t feat, int reduce, const int64_t* long_rows,
                                   const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks,
                                   int64_t chunk, float* partials, int idx_dtype, int val_dtype, void* stream) {
     B200MP_CHECK_ARG(n_rows >= 0 && n_src >= 0 && feat >= 0);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(ptr && out);
     B200MP_CHECK_ARG(src || n_src == 0);
-    B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && partials && chunk > 0));
-    LongRowPlan plan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, partials,
-                     nullptr, 0, 0, nullptr, 0};
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) return segment_typed<float, int32_t>(ptr, src, out, n_rows, feat, reduce, plan, s);
-    if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) return segment_typed<float, int64_t>(ptr, src, out, n_rows, feat, reduce, plan, s);
-    if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) return segment_typed<__nv_bfloat16, int32_t>(ptr, src, out, n_rows, feat, reduce, plan, s);
-    if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) return segment_typed<__nv_bfloat16, int64_t>(ptr, src, out, n_rows, feat, reduce, plan, s);
-    set_error("segment_csr: unsupported dtype combination val=%d idx=%d", val_dtype, idx_dtype);
-    return B200MP_ERR_UNSUPPORTED;
+    return dispatch_val_idx(val_dtype, idx_dtype, "segment_csr", [&](auto tv, auto ti) {
+        using T = decltype(tv);
+        using I = decltype(ti);
+        return csr_reduce_auto<T, I, false>(static_cast<const I*>(ptr), static_cast<const I*>(nullptr), nullptr,
+                                             static_cast<const T*>(src), static_cast<T*>(out), n_rows, feat, reduce,
+                                             true, plan, nullptr, static_cast<cudaStream_t>(stream));
+    });
 }

@@ -147,13 +147,6 @@ __device__ __forceinline__ void sm_store_gt(const float* sh, int groups, int64_t
     }
 }
 
-template <int EPV>
-__device__ __forceinline__ void sm_store_part(float* p, const float (&v)[EPV]) {
-#pragma unroll
-    for (int j = 0; j < EPV / 4; ++j)
-        *reinterpret_cast<float4*>(p + 4 * j) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-}
-
 // ---------------------------------------------------------------- the three sweeps, 16-byte vector path
 template <typename T, typename I, int MODE, int FORM, int TMODE, bool WANT_T>
 __global__ void __launch_bounds__(128)
@@ -289,10 +282,10 @@ softmax_aggr_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, SmA
         }
         if (is_chunk) {
             constexpr int NACC = MODE == kSmFwd ? 3 : 1;
-            sm_store_part<EPV>(plan.partials + static_cast<size_t>(item * NACC) * F + f0, acc0);
+            store_partial<EPV>(plan.partials + static_cast<size_t>(item * NACC) * F + f0, acc0);
             if (MODE == kSmFwd) {
-                sm_store_part<EPV>(plan.partials + static_cast<size_t>(item * NACC + 1) * F + f0, acc1);
-                sm_store_part<EPV>(plan.partials + static_cast<size_t>(item * NACC + 2) * F + f0, acc2);
+                store_partial<EPV>(plan.partials + static_cast<size_t>(item * NACC + 1) * F + f0, acc1);
+                store_partial<EPV>(plan.partials + static_cast<size_t>(item * NACC + 2) * F + f0, acc2);
             }
             continue;
         }
@@ -302,7 +295,7 @@ softmax_aggr_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, SmA
 #pragma unroll
             for (int i = 0; i < EPV; ++i) sm_final(acc0[i], acc1[i], acc2[i], end > begin, f[i], l[i]);
             stg_stream16(dst, ElemTraits<T>::pack(f));
-            if (args.lse) sm_store_part<EPV>(args.lse + row * F + f0, l);
+            if (args.lse) store_partial<EPV>(args.lse + row * F + f0, l);
         } else {
             stg_stream16(dst, ElemTraits<T>::pack(acc0));
         }
@@ -506,25 +499,6 @@ int sm_typed(const void* rowptr_, const void* col_, SmArgs args, int form, int t
     return B200MP_ERR_INVALID_ARG;
 }
 
-template <typename T, typename I>
-int sm_fwd_typed(const void* r, const void* c, SmArgs a, int form, int tm, bool wt, int64_t n, LongRowPlan p, cudaStream_t s) {
-    return sm_typed<T, I, kSmFwd>(r, c, a, form, tm, wt, n, p, s);
-}
-template <typename T, typename I>
-int sm_dst_typed(const void* r, const void* c, SmArgs a, int form, int tm, bool wt, int64_t n, LongRowPlan p, cudaStream_t s) {
-    return sm_typed<T, I, kSmDst>(r, c, a, form, tm, wt, n, p, s);
-}
-template <typename T, typename I>
-int sm_src_typed(const void* r, const void* c, SmArgs a, int form, int tm, bool wt, int64_t n, LongRowPlan p, cudaStream_t s) {
-    return sm_typed<T, I, kSmSrc>(r, c, a, form, tm, wt, n, p, s);
-}
-
-inline LongRowPlan sm_plan(const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks,
-                           int64_t chunk, float* partials) {
-    return LongRowPlan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, partials,
-                       nullptr, 0, 0, nullptr, 0, nullptr};
-}
-
 // Message form from the operands: x and / or a, identity or relu + eps.
 inline int sm_form(const void* x, const void* a, int message) {
     if (message == 1) return a ? kSmXARelu : kSmXRelu;
@@ -535,23 +509,11 @@ inline int sm_form(const void* x, const void* a, int message) {
 
 using namespace b200mp;
 
-#define DISPATCH_T_I(FN, ...)                                                                                   \
-    do {                                                                                                        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) return FN<float, int32_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) return FN<float, int64_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) return FN<__nv_bfloat16, int32_t>(__VA_ARGS__); \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) return FN<__nv_bfloat16, int64_t>(__VA_ARGS__); \
-        set_error("unsupported dtype combination val=%d idx=%d", val_dtype, idx_dtype);                         \
-        return B200MP_ERR_UNSUPPORTED;                                                                          \
-    } while (0)
-
 #define B200MP_CHECK_SM()                                                                                       \
     B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0);                                  \
     B200MP_CHECK_ARG(message == 0 || message == 1);                                                             \
     B200MP_CHECK_ARG(t_mode >= 0 && t_mode <= 2 && (t_mode == 0 || t));                                        \
-    B200MP_CHECK_ARG(message == 1 ? x != nullptr : (x == nullptr) != (edge_rows == nullptr));                  \
-    B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);                                                        \
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && partials && chunk > 0))
+    B200MP_CHECK_ARG(message == 1 ? x != nullptr : (x == nullptr) != (edge_rows == nullptr))
 
 extern "C" int b200mp_softmax_aggr_csr(const void* rowptr, const void* col, const void* perm, const void* x,
                                        const void* edge_rows, const float* t, void* out, float* lse, int64_t n_rows,
@@ -560,12 +522,16 @@ extern "C" int b200mp_softmax_aggr_csr(const void* rowptr, const void* col, cons
                                        int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials,
                                        int idx_dtype, int val_dtype, void* stream) {
     B200MP_CHECK_SM();
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && out);
     B200MP_CHECK_ARG(n_edges == 0 || x == nullptr || col);
     const SmArgs a{x, edge_rows, t, perm, nullptr, nullptr, lse, out, nullptr, feat, eps, false};
-    DISPATCH_T_I(sm_fwd_typed, rowptr, col, a, sm_form(x, edge_rows, message), t_mode, false, n_rows,
-                 sm_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials), static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "softmax_aggr_csr", [&](auto tv, auto ti) {
+        return sm_typed<decltype(tv), decltype(ti), kSmFwd>(rowptr, col, a, sm_form(x, edge_rows, message), t_mode, false,
+                                                          n_rows, plan, static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int64_t b200mp_softmax_aggr_workspace(int64_t n_rows, int64_t n_chunks, int64_t feat) {
@@ -581,7 +547,7 @@ int sm_dst_with_t(const void* rowptr, const void* col, SmArgs a, int form, int t
     bool vec;
     const int64_t ctas = sm_grid<T>(a, plan, n_rows, lg, vec);
     a.gt_part = ws;
-    const int rc = sm_dst_typed<T, I>(rowptr, col, a, form, t_mode, grad_t != nullptr, n_rows, plan, s);
+    const int rc = sm_typed<T, I, kSmDst>(rowptr, col, a, form, t_mode, grad_t != nullptr, n_rows, plan, s);
     if (rc != B200MP_OK || grad_t == nullptr) return rc;
     if (ctas == 0) return cudaMemsetAsync(grad_t, 0, a.feat * sizeof(float), s) == cudaSuccess ? B200MP_OK : B200MP_ERR_CUDA;
     return b200mp_column_sum(ws, grad_t, ws + ctas * a.feat, b200mp_column_sum_parts(ctas), ctas, a.feat, B200MP_F32, s);
@@ -595,14 +561,10 @@ extern "C" int b200mp_softmax_aggr_backward_dst(const void* rowptr, const void* 
                                                 int semi_grad, const int64_t* long_rows, const int64_t* chunk_ptr,
                                                 int64_t n_long_rows, int64_t n_chunks, int64_t chunk, int idx_dtype,
                                                 int val_dtype, void* stream) {
-    float* partials = nullptr;
-    B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0);
-    B200MP_CHECK_ARG(message == 0 || message == 1);
-    B200MP_CHECK_ARG(t_mode >= 0 && t_mode <= 2 && (t_mode == 0 || t));
-    B200MP_CHECK_ARG(message == 1 ? x != nullptr : (x == nullptr) != (edge_rows == nullptr));
-    B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && chunk > 0));
+    B200MP_CHECK_SM();
     B200MP_CHECK_ARG(grad_t == nullptr || (t_mode != 0 && workspace));
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, nullptr, false)) return rc;
     if (feat == 0) return B200MP_OK;
     if (n_rows == 0) {
         if (grad_t) return cudaMemsetAsync(grad_t, 0, feat * sizeof(float), static_cast<cudaStream_t>(stream)) == cudaSuccess
@@ -613,8 +575,10 @@ extern "C" int b200mp_softmax_aggr_backward_dst(const void* rowptr, const void* 
     B200MP_CHECK_ARG(n_edges == 0 || x == nullptr || col);
     const SmArgs a{x, edge_rows, t, perm, grad_out, out, const_cast<float*>(lse), grad_edge_rows, nullptr, feat, eps,
                    semi_grad != 0};
-    DISPATCH_T_I(sm_dst_with_t, rowptr, col, a, sm_form(x, edge_rows, message), t_mode, grad_t, workspace, n_rows,
-                 sm_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials), static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "softmax_aggr_backward_dst", [&](auto tv, auto ti) {
+        return sm_dst_with_t<decltype(tv), decltype(ti)>(rowptr, col, a, sm_form(x, edge_rows, message), t_mode, grad_t,
+                                                       workspace, n_rows, plan, static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int b200mp_softmax_aggr_backward_src(const void* rowptr_t, const void* col_t, const void* perm_t,
@@ -628,11 +592,15 @@ extern "C" int b200mp_softmax_aggr_backward_src(const void* rowptr_t, const void
     const int64_t n_rows = n_src, n_cols = n_dst;
     B200MP_CHECK_SM();
     B200MP_CHECK_ARG(x != nullptr);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_src == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr_t && grad_x);
     B200MP_CHECK_ARG(n_edges == 0 || (col_t && out && lse && grad_out && (edge_rows == nullptr || perm_t)));
     const SmArgs a{x, edge_rows, t, perm_t, grad_out, out, const_cast<float*>(lse), grad_x, nullptr, feat, eps,
                    semi_grad != 0};
-    DISPATCH_T_I(sm_src_typed, rowptr_t, col_t, a, sm_form(x, edge_rows, message), t_mode, false, n_src,
-                 sm_plan(long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials), static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "softmax_aggr_backward_src", [&](auto tv, auto ti) {
+        return sm_typed<decltype(tv), decltype(ti), kSmSrc>(rowptr_t, col_t, a, sm_form(x, edge_rows, message), t_mode,
+                                                          false, n_src, plan, static_cast<cudaStream_t>(stream));
+    });
 }

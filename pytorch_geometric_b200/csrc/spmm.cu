@@ -101,15 +101,6 @@ sddmm_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, const T* _
     }
 }
 
-template <typename T, typename I>
-int spmm_typed(const void* rowptr, const void* col, const float* val, const void* x, void* out,
-               int64_t n_rows, int64_t feat, int reduce, LongRowPlan plan, const float* bias,
-               cudaStream_t stream) {
-    return csr_reduce_auto<T, I, true>(static_cast<const I*>(rowptr), static_cast<const I*>(col), val,
-                                        static_cast<const T*>(x), static_cast<T*>(out), n_rows, feat,
-                                        reduce, false, plan, bias, stream);
-}
-
 inline int group_width(int64_t feat) {
     int g = 1;
     while (g < 32 && g < feat) g <<= 1;
@@ -119,16 +110,6 @@ inline int group_width(int64_t feat) {
 }  // namespace b200mp
 
 using namespace b200mp;
-
-#define DISPATCH_T_I(FN, ...)                                                        \
-    do {                                                                             \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I32) return FN<float, int32_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_F32 && idx_dtype == B200MP_I64) return FN<float, int64_t>(__VA_ARGS__);        \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I32) return FN<__nv_bfloat16, int32_t>(__VA_ARGS__); \
-        if (val_dtype == B200MP_BF16 && idx_dtype == B200MP_I64) return FN<__nv_bfloat16, int64_t>(__VA_ARGS__); \
-        set_error("unsupported dtype combination val=%d idx=%d", val_dtype, idx_dtype);                         \
-        return B200MP_ERR_UNSUPPORTED;                                                                          \
-    } while (0)
 
 extern "C" int b200mp_spmm_csr(const void* rowptr, const void* col, const float* val, const void* x,
                                void* out, int64_t n_rows, int64_t n_cols, int64_t feat, int reduce,
@@ -140,6 +121,8 @@ extern "C" int b200mp_spmm_csr(const void* rowptr, const void* col, const float*
     B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && feat >= 0);
     B200MP_CHECK_ARG((flags & ~1) == 0 && (!(flags & 1) || (reduce == B200MP_SUM && !bias)));
     B200MP_CHECK_ARG(!relu_mask || (flags & 1));
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && out);
     B200MP_CHECK_ARG(x || n_cols == 0 || peer_ptrs);
@@ -147,52 +130,21 @@ extern "C" int b200mp_spmm_csr(const void* rowptr, const void* col, const float*
     // the scalar fallback, taken when a matrix is not 16-byte aligned, has no peer-table addressing
     B200MP_CHECK_ARG(!peer_ptrs || (aligned16(x) && aligned16(out) && aligned16(relu_mask) &&
                                     (n_long_rows == 0 || aligned16(partials))));
-    B200MP_CHECK_ARG(n_long_rows >= 0 && n_chunks >= 0);
-    B200MP_CHECK_ARG(n_long_rows == 0 || (long_rows && chunk_ptr && partials && chunk > 0));
     B200MP_CHECK_ARG(!x_halo || (n_local_cols >= 0 && n_local_cols <= n_cols));
-    LongRowPlan plan{long_rows, chunk_ptr, n_long_rows, n_long_rows ? n_chunks : 0, chunk, partials,
-                     x_halo, x_halo ? n_local_cols : 0, flags & 1,
-                     static_cast<const unsigned long long*>(peer_ptrs), peer_ptrs ? peer_rows : 0, relu_mask};
-    DISPATCH_T_I(spmm_typed, rowptr, col, val, x, out, n_rows, feat, reduce, plan, bias,
-                 static_cast<cudaStream_t>(stream));
+    plan.x2 = x_halo;
+    plan.split = x_halo ? n_local_cols : 0;
+    plan.accumulate = flags & 1;
+    plan.peers = static_cast<const unsigned long long*>(peer_ptrs);
+    plan.peer_rows = peer_ptrs ? peer_rows : 0;
+    plan.relu_mask = relu_mask;
+    return dispatch_val_idx(val_dtype, idx_dtype, "spmm_csr", [&](auto tv, auto ti) {
+        using T = decltype(tv);
+        using I = decltype(ti);
+        return csr_reduce_auto<T, I, true>(static_cast<const I*>(rowptr), static_cast<const I*>(col), val,
+                                            static_cast<const T*>(x), static_cast<T*>(out), n_rows, feat, reduce,
+                                            false, plan, bias, static_cast<cudaStream_t>(stream));
+    });
 }
-
-namespace b200mp {
-template <typename T, typename I>
-int ties_typed(const void* rowptr, const void* col, const float* val, const void* x, const void* out,
-               float* ties, int64_t n_rows, int64_t feat, int count_self_zero, cudaStream_t stream) {
-    const int g = group_width(feat);
-    const int64_t blocks = ceil_div(n_rows, 256 / g);
-    minmax_ties_kernel<T, I><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
-        static_cast<const I*>(rowptr), static_cast<const I*>(col), val, static_cast<const T*>(x),
-        static_cast<const T*>(out), ties, n_rows, feat, g, count_self_zero != 0);
-    B200MP_LAUNCH_CHECK();
-    return B200MP_OK;
-}
-template <typename T, typename I>
-int mmbwd_typed(const void* rowptr_t, const void* col_t, const float* val_t, const void* x,
-                const void* out, const void* grad_out, const float* ties, void* grad_x, int64_t n_src,
-                int64_t feat, cudaStream_t stream) {
-    const int g = group_width(feat);
-    const int64_t blocks = ceil_div(n_src, 256 / g);
-    minmax_backward_kernel<T, I><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
-        static_cast<const I*>(rowptr_t), static_cast<const I*>(col_t), val_t, static_cast<const T*>(x),
-        static_cast<const T*>(out), static_cast<const T*>(grad_out), ties, static_cast<T*>(grad_x), n_src,
-        feat, g);
-    B200MP_LAUNCH_CHECK();
-    return B200MP_OK;
-}
-template <typename T, typename I>
-int sddmm_typed(const void* rowptr, const void* col, const void* a, const void* b, float* dot,
-                int64_t n_rows, int64_t feat, cudaStream_t stream) {
-    const int64_t blocks = ceil_div(n_rows, 8);
-    sddmm_kernel<T, I><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
-        static_cast<const I*>(rowptr), static_cast<const I*>(col), static_cast<const T*>(a),
-        static_cast<const T*>(b), dot, n_rows, feat);
-    B200MP_LAUNCH_CHECK();
-    return B200MP_OK;
-}
-}  // namespace b200mp
 
 extern "C" int b200mp_minmax_ties(const void* rowptr, const void* col, const float* val, const void* x,
                                   const void* out, float* ties, int64_t n_rows, int64_t feat,
@@ -200,8 +152,17 @@ extern "C" int b200mp_minmax_ties(const void* rowptr, const void* col, const flo
     B200MP_CHECK_ARG(n_rows >= 0 && feat >= 0);
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && out && ties);
-    DISPATCH_T_I(ties_typed, rowptr, col, val, x, out, ties, n_rows, feat, count_self_zero,
-                 static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "minmax_ties", [&](auto tv, auto ti) {
+        using T = decltype(tv);
+        using I = decltype(ti);
+        const int g = group_width(feat);
+        minmax_ties_kernel<T, I><<<static_cast<unsigned>(ceil_div(n_rows, 256 / g)), 256, 0,
+                                   static_cast<cudaStream_t>(stream)>>>(
+            static_cast<const I*>(rowptr), static_cast<const I*>(col), val, static_cast<const T*>(x),
+            static_cast<const T*>(out), ties, n_rows, feat, g, count_self_zero != 0);
+        B200MP_LAUNCH_CHECK();
+        return B200MP_OK;
+    });
 }
 
 extern "C" int b200mp_minmax_backward(const void* rowptr_t, const void* col_t, const float* val_t,
@@ -211,8 +172,18 @@ extern "C" int b200mp_minmax_backward(const void* rowptr_t, const void* col_t, c
     B200MP_CHECK_ARG(n_src >= 0 && feat >= 0);
     if (n_src == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr_t && x && grad_x);
-    DISPATCH_T_I(mmbwd_typed, rowptr_t, col_t, val_t, x, out, grad_out, ties, grad_x, n_src, feat,
-                 static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "minmax_backward", [&](auto tv, auto ti) {
+        using T = decltype(tv);
+        using I = decltype(ti);
+        const int g = group_width(feat);
+        minmax_backward_kernel<T, I><<<static_cast<unsigned>(ceil_div(n_src, 256 / g)), 256, 0,
+                                       static_cast<cudaStream_t>(stream)>>>(
+            static_cast<const I*>(rowptr_t), static_cast<const I*>(col_t), val_t, static_cast<const T*>(x),
+            static_cast<const T*>(out), static_cast<const T*>(grad_out), ties, static_cast<T*>(grad_x), n_src,
+            feat, g);
+        B200MP_LAUNCH_CHECK();
+        return B200MP_OK;
+    });
 }
 
 extern "C" int b200mp_sddmm_csr(const void* rowptr, const void* col, const void* a, const void* b,
@@ -221,5 +192,13 @@ extern "C" int b200mp_sddmm_csr(const void* rowptr, const void* col, const void*
     B200MP_CHECK_ARG(n_rows >= 0 && feat >= 0);
     if (n_rows == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && dot);
-    DISPATCH_T_I(sddmm_typed, rowptr, col, a, b, dot, n_rows, feat, static_cast<cudaStream_t>(stream));
+    return dispatch_val_idx(val_dtype, idx_dtype, "sddmm_csr", [&](auto tv, auto ti) {
+        using T = decltype(tv);
+        using I = decltype(ti);
+        sddmm_kernel<T, I><<<static_cast<unsigned>(ceil_div(n_rows, 8)), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+            static_cast<const I*>(rowptr), static_cast<const I*>(col), static_cast<const T*>(a),
+            static_cast<const T*>(b), dot, n_rows, feat);
+        B200MP_LAUNCH_CHECK();
+        return B200MP_OK;
+    });
 }

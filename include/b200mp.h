@@ -358,6 +358,61 @@ int b200mp_softmax_aggr_backward_src(const void* rowptr_t, const void* col_t, co
                                      int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials,
                                      int idx_dtype, int val_dtype, void* stream);
 
+/* ------------------------------------------------------------------ power-mean aggregation (one sweep)
+ * Per destination i, feature f, in-edge e = (j -> i) in [rowptr[i], rowptr[i+1]), eid(e) = perm[e] or e (perm NULL),
+ * with m_e formed as in b200mp_softmax_aggr_csr (message 0: x[col[e]] | edge_rows[eid(e)]; message 1:
+ * relu(x[col[e]] (+ edge_rows[eid(e)])) + eps, each step rounded):
+ *   c_e = clamp(m_e, clamp_min, clamp_max)   y_e = c_e ^ p (rounded)   M_i = sum_e y_e / max(deg_i, 1) (rounded)
+ *   out[i, f] = clamp(M_i, clamp_min, clamp_max) ^ (1 / p) (rounded)
+ * p_mode 0: no clamp and no pow (a plain mean of the messages); 1: p[0]; 2: p[f].  p is fp32 on the device (a learnable
+ * p costs no host read); 1 / p is formed in fp32.  With p: clamp_min > 0 and clamp_max >= clamp_min (+inf: no upper
+ * bound); the clamp keeps NaN.  An empty row gives clamp_min ^ (1 / p) with p and 0 without.  c ^ p is
+ * ex2.approx(p lg2.approx(c)) (csrc/power_mean.cu states the bound); the sum is fp32 and compensated.
+ * Replaces: PowerMeanAggregation.forward (nn/aggr/basic.py:275-293: clamp, pow, scatter mean, clamp, pow over [E, F]),
+ * behind GENConv.message (nn/conv/gen_conv.py:231-239) with message 1.
+ * x: [n_cols, feat]; edge_rows: [n_edges, feat] in the CALLER's edge order; out: [n_rows, feat]; mean: NULL or
+ * [n_rows, feat] fp32 = M, the only state the backward needs.  Long rows: plan as in b200mp_spmm_csr, partials
+ * [n_chunks, feat] fp32, summed in chunk order by a second launch. */
+int b200mp_power_mean_csr(const void* rowptr, const void* col, const void* perm, const void* x,
+                          const void* edge_rows, const float* p, void* out, float* mean, int64_t n_rows,
+                          int64_t n_cols, int64_t n_edges, int64_t feat, int message, float eps, int p_mode,
+                          float clamp_min, float clamp_max, const int64_t* plan_long_rows, const int64_t* plan_chunk_ptr,
+                          int64_t plan_n_long_rows, int64_t plan_n_chunks, int64_t plan_chunk, float* plan_partials, int idx_dtype,
+                          int val_dtype, void* stream);
+/* fp32 workspace elements of the power-mean backward: b200mp_power_mean_backward_dst over n_rows destination rows
+ * (n_node = 0), or b200mp_power_mean_backward_src over n_rows source rows of the transposed CSR with n_node = n_dst
+ * (its node plane). */
+int64_t b200mp_power_mean_workspace(int64_t n_node, int64_t n_rows, int64_t plan_n_chunks, int64_t feat);
+/* Destination sweep of the backward (replaces the autograd of basic.py:275-293 / gen_conv.py:231-239 over [E, F]).
+ * Recomputes m, c and y; with g = grad_out[i], o = out[i] and C_i = clamp(M_i):
+ *   G_i = g (1/p) C_i ^ (1/p - 1) / max(deg_i, 1) [clamp_min <= M_i <= clamp_max]   (p_mode 0: g / max(deg_i, 1))
+ *   grad_m_e = G_i p c_e ^ (p - 1) [clamp_min <= m_e <= clamp_max]     grad_s_e = grad_m_e [s_e > 0 or NaN] (message 1)
+ *   grad_edge_rows[eid(e)] = grad_s_e (NULL: not written)
+ *   grad_p[f] = sum_i sum_e G_i y_e ln c_e - sum_i g o ln C_i / p^2     (the second sum includes empty rows)
+ * grad_p: NULL or [feat] fp32 (per-channel sums; the caller sums them for a scalar p), from per-CTA partials folded in
+ * fixed order by b200mp_column_sum in `workspace` (b200mp_power_mean_workspace(0, n_rows, plan_n_chunks, feat)). */
+int b200mp_power_mean_backward_dst(const void* rowptr, const void* col, const void* perm, const void* x,
+                                   const void* edge_rows, const float* p, const void* out, const float* mean,
+                                   const void* grad_out, void* grad_edge_rows, float* grad_p, float* workspace,
+                                   int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t feat, int message,
+                                   float eps, int p_mode, float clamp_min, float clamp_max, const int64_t* plan_long_rows,
+                                   const int64_t* plan_chunk_ptr, int64_t plan_n_long_rows, int64_t plan_n_chunks, int64_t plan_chunk,
+                                   int idx_dtype, int val_dtype, void* stream);
+/* grad_x (and grad_p) by ONE sweep over the TRANSPOSED CSR: a node kernel first writes G_i of every destination into
+ * `workspace` (b200mp_power_mean_workspace(n_dst, n_src, plan_n_chunks, feat)) with the per-row grad_p terms, then
+ * grad_x[j] = sum_{t in rowT(j)} grad_s_t gathers one fp32 row of G at col_t[t] and edge_rows[perm_t[t]] (frozen edge
+ * rows) per out-edge.  rowptr: the destination CSR's (for the degrees).  Needs x.  Used when no grad_edge_rows was
+ * written; otherwise the segment sum of grad_edge_rows over the transposed CSR (b200mp_spmm_csr with perm_t as the
+ * column) gives grad_x with fewer bytes.  Long source rows: the transposed CSR's plan, partials [plan_n_chunks, feat]. */
+int b200mp_power_mean_backward_src(const void* rowptr, const void* rowptr_t, const void* col_t, const void* perm_t,
+                                   const void* x, const void* edge_rows, const float* p, const void* out,
+                                   const float* mean, const void* grad_out, void* grad_x, float* grad_p,
+                                   float* workspace, int64_t n_src, int64_t n_dst, int64_t n_edges, int64_t feat,
+                                   int message, float eps, int p_mode, float clamp_min, float clamp_max,
+                                   const int64_t* plan_long_rows, const int64_t* plan_chunk_ptr, int64_t plan_n_long_rows,
+                                   int64_t plan_n_chunks, int64_t plan_chunk, float* plan_partials, int idx_dtype, int val_dtype,
+                                   void* stream);
+
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)
  * out[index[e], :] (+)= src[e, :] for an UNSORTED index.  Replaces utils/_scatter.py:14-138
  * (aten::scatter_add_ / scatter_reduce_, torch_scatter.scatter).  fp32 only.  `count` is a

@@ -59,6 +59,13 @@ _SIGS = {
                                                                            _INT, _INT, _P]),
     "b200mp_softmax_aggr_backward_src": (_INT, [_P] * 10 + [_I64] * 4 + [_INT, _F, _INT, _INT, _P, _P, _I64, _I64, _I64,
                                                                            _P, _INT, _INT, _P]),
+    "b200mp_power_mean_csr": (_INT, [_P] * 8 + [_I64] * 4 + [_INT, _F, _INT, _F, _F, _P, _P, _I64, _I64, _I64, _P,
+                                                              _INT, _INT, _P]),
+    "b200mp_power_mean_workspace": (_I64, [_I64, _I64, _I64, _I64]),
+    "b200mp_power_mean_backward_dst": (_INT, [_P] * 12 + [_I64] * 4 + [_INT, _F, _INT, _F, _F, _P, _P, _I64, _I64, _I64,
+                                                                         _INT, _INT, _P]),
+    "b200mp_power_mean_backward_src": (_INT, [_P] * 13 + [_I64] * 4 + [_INT, _F, _INT, _F, _F, _P, _P, _I64, _I64, _I64,
+                                                                         _P, _INT, _INT, _P]),
     "b200mp_scatter_coo": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
     "b200mp_split_tf32": (_INT, [_P, _P, _P, _I64, _P]),
     "b200mp_split_tf32_transposed": (_INT, [_P, _P, _P, _I64, _I64, _P]),

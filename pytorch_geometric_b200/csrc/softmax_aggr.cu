@@ -24,6 +24,7 @@
 // Mapping as in cg.cu: a lane group of G lanes per row (runtime power of two), one 16-byte vector per lane and trip,
 // rows longer than the plan's chunk split into chunks whose fp32 partials a combine kernel folds in chunk order.
 // Rows that are not a whole number of aligned 16-byte vectors take a one-warp scalar kernel.
+#include "aggr_message.cuh"
 #include "csr_reduce.cuh"
 #include "gate_math.cuh"
 
@@ -34,7 +35,6 @@ extern "C" int64_t b200mp_column_sum_parts(int64_t n_rows);
 namespace b200mp {
 
 enum SmMode { kSmFwd = 0, kSmDst = 1, kSmSrc = 2 };
-enum SmForm { kSmX = 0, kSmA = 1, kSmXRelu = 2, kSmXARelu = 3 };   // which rows are read, and the message
 enum SmT { kSmTNone = 0, kSmTScalar = 1, kSmTChannel = 2 };
 
 struct SmArgs {
@@ -51,22 +51,6 @@ struct SmArgs {
     float eps;
     bool semi;
 };
-
-template <int FORM>
-struct SmForms {
-    static constexpr bool kX = FORM != kSmA;
-    static constexpr bool kA = FORM == kSmA || FORM == kSmXARelu;
-    static constexpr bool kRelu = FORM == kSmXRelu || FORM == kSmXARelu;
-};
-
-// The message m and its pre-activation gate `on` from the fp32 loads.
-template <typename T, int FORM>
-__device__ __forceinline__ float sm_message(float xv, float av, float eps, bool& on) {
-    using Fm = SmForms<FORM>;
-    const float s = (Fm::kX && Fm::kA) ? round_to<T>(__fadd_rn(xv, av)) : (Fm::kX ? xv : av);
-    on = !(s <= 0.0f);
-    return Fm::kRelu ? round_to<T>(__fadd_rn(on ? s : 0.0f, eps)) : s;
-}
 
 template <typename T, int TMODE>
 __device__ __forceinline__ float sm_logit(float m, float tv) {
@@ -497,12 +481,6 @@ int sm_typed(const void* rowptr_, const void* col_, SmArgs args, int form, int t
     }
     set_error("softmax_aggr: the transposed sweep needs x");
     return B200MP_ERR_INVALID_ARG;
-}
-
-// Message form from the operands: x and / or a, identity or relu + eps.
-inline int sm_form(const void* x, const void* a, int message) {
-    if (message == 1) return a ? kSmXARelu : kSmXRelu;
-    return x ? kSmX : kSmA;
 }
 
 }  // namespace b200mp

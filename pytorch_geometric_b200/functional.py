@@ -373,6 +373,83 @@ def softmax_aggregate(graph, x: Optional[Tensor], a: Optional[Tensor] = None, t=
     return _SoftmaxAggregate.apply(x, a, tt, where, float(eps), message, bool(semi_grad), want_lse)
 
 
+class _PowerMeanAggregate(torch.autograd.Function):
+    """clamp(mean_e clamp(m_e)^p)^(1/p) per destination and feature (csrc/power_mean.cu).  The only saved state is
+    the fp32 plane of the means; the backward recomputes m, c and y.  The destination sweep gives grad_a and grad_p;
+    grad_x is then the segment sum of grad_a's rows over the transposed CSR, and otherwise one transposed sweep (which
+    then gives grad_p).  Each sweep runs only when one of its outputs is needed."""
+
+    @staticmethod
+    def forward(ctx, x, a, p, where, eps: float, message: str, lo: float, hi, want_mean: bool):
+        rowptr, col, perm, plan, n_edges, _ = where
+        out, mean = ops.power_mean_csr(rowptr, col, perm, x, a, p, rowptr.numel() - 1, n_edges, message, eps, lo, hi,
+                                       plan, want_mean and p is not None)
+        ctx.where, ctx.eps, ctx.message, ctx.lo, ctx.hi = where, eps, message, lo, hi
+        ctx.save_for_backward(x, a, p, out, mean)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out: Tensor):
+        x, a, p, out, mean = ctx.saved_tensors
+        rowptr, col, perm, plan, n_edges, graph = ctx.where
+        need_x, need_a, need_p = ctx.needs_input_grad[:3]
+        gx = ga = gp = None
+        if need_a or (need_p and not need_x):
+            ga, gp = ops.power_mean_backward_dst(rowptr, col, perm, x, a, p, out, mean, grad_out, n_edges, ctx.message,
+                                                 ctx.eps, ctx.lo, ctx.hi, need_a, need_p, plan)
+        if need_x:
+            graph.build_transpose()
+            if ga is not None:
+                # grad_x[j] = the sum of grad_a over j's out-edges: perm_t is the caller's edge id of each transposed slot
+                gx = ops.spmm_csr(graph.rowptr_t, graph.perm_t, None, ga, graph.num_src, "sum", graph.plan_t)
+            else:
+                gx, gp = ops.power_mean_backward_src(rowptr, graph.rowptr_t, graph.col_t, graph.perm_t, x, a, p, out,
+                                                     mean, grad_out, ctx.message, ctx.eps, ctx.lo, ctx.hi, need_p,
+                                                     graph.plan_t)
+        if gp is not None:
+            gp = gp.sum().view(1) if p.numel() == 1 else gp
+        return gx, ga, gp, None, None, None, None, None, None
+
+
+def power_mean_aggregate(graph, x: Optional[Tensor], a: Optional[Tensor] = None, p=1.0, eps: float = 0.0,
+                         message: str = "identity", clamp_min: float = 1e-4,
+                         clamp_max: Optional[float] = 100.0) -> Tensor:
+    """PowerMeanAggregation (nn/aggr/basic.py:275-293), optionally behind GENConv's message relu(x_j + e_ji) + eps
+    (gen_conv.py:231-239), in one sweep with nothing stored per edge:
+
+        m_e = x[j] | a[e] | relu(x[j] (+ a[e])) + eps,
+        out[i] = clamp(mean_{e = (j -> i)} clamp(m_e, clamp_min, clamp_max) ^ p, clamp_min, clamp_max) ^ (1 / p)
+
+    graph, x, a and message as in softmax_aggregate.  p: a Python number (1 skips both clamps and both pows, as the
+    reference does: a plain mean) or a tensor of 1 or F elements whose values the kernel reads on the device in fp32,
+    so a learnable p adds no host sync; p's gradient has p's shape and dtype.  With p, clamp_min must be positive and
+    clamp_max may be None (no upper bound).  An empty row gives clamp_min ^ (1 / p), or 0 without p."""
+    if isinstance(graph, CSRGraph):
+        where = (graph.rowptr, graph.col, graph.perm, graph.plan, graph.num_edges, graph)
+        if x is not None and x.size(0) != graph.num_src:
+            raise ValueError(f"x has {x.size(0)} rows but the graph has {graph.num_src} source nodes")
+    else:
+        if x is not None:
+            raise ValueError("a (ptr, plan) message layout takes the messages as `a`, not x")
+        ptr, plan = graph
+        where = (ptr, None, None, plan, a.size(0), None)
+    ref = x if x is not None else a
+    if ref is None or ref.dim() != 2:
+        raise ValueError("power_mean_aggregate takes two-dimensional x or a")
+    if isinstance(p, Tensor):
+        pp = p.reshape(-1).float().contiguous()
+        if pp.numel() not in (1, ref.size(1)):
+            raise ValueError(f"p must have 1 or {ref.size(1)} elements, got {p.numel()}")
+    elif float(p) == 1.0:
+        pp = None                                                          # basic.py:285,290: no clamp, no pow
+    else:
+        pp = torch.full((1, ), float(p), dtype=torch.float32, device=ref.device)   # ATen's fp32 scalar
+    x = None if x is None else x.contiguous()
+    a = None if a is None else a.contiguous()
+    want_mean = torch.is_grad_enabled() and any(v is not None and v.requires_grad for v in (x, a, pp))
+    return _PowerMeanAggregate.apply(x, a, pp, where, float(eps), message, clamp_min, clamp_max, want_mean)
+
+
 class _PNAAggregate(torch.autograd.Function):
     """PNAConv's aggregation of m_e = u_i + w_e, w_e = v_j (+ c_e) (csrc/pna.cu).  The sweep collects the statistics
     of w (b200mp_multi_aggr_csr on v, or b200mp_pna_edge_stats with c); the epilogue shifts them by u, applies the

@@ -1,5 +1,5 @@
-"""Aggregation modules: mirrors of torch_geometric.nn.aggr.{Sum,Mean,Max,Min,Var,Std,Softmax}Aggregation
-(nn/aggr/base.py:102-185, basic.py:12-50,83-139,142-218), FusedAggregation (fused.py:20-336) and
+"""Aggregation modules: mirrors of torch_geometric.nn.aggr.{Sum,Mean,Max,Min,Var,Std,Softmax,PowerMean}Aggregation
+(nn/aggr/base.py:102-185, basic.py:12-50,83-139,142-297), FusedAggregation (fused.py:20-336) and
 MultiAggregation (multi.py:14-200) on the sm_90a kernels.
 
 `__call__(x, index=None, ptr=None, dim_size=None, dim=-2)` has the reference's meaning and error
@@ -163,6 +163,89 @@ def _softmax_forward(x, t, semi_grad, index, ptr, dim_size, index_sorted):
     return Fn.softmax_aggregate(CSRGraph(e, index, index.numel(), dim_size), None, x, t, semi_grad=semi_grad)
 
 
+class PowerMeanAggregation(Aggregation):
+    """out = clamp(mean(clamp(x)^p))^(1/p) per group   (nn/aggr/basic.py:221-297), as one sweep over the messages
+    (functional.power_mean_aggregate): no [E, F] intermediate is stored, and a learnable p is read on the device."""
+
+    def __init__(self, p: float = 1.0, learn: bool = False, channels: int = 1, clamp_min: Optional[float] = 1e-4,
+                 clamp_max: Optional[float] = 100.):
+        super().__init__()
+        if not learn and channels != 1:
+            raise ValueError(f"Cannot set 'channels' greater than '1' in case '{self.__class__.__name__}' is not "
+                             f"trainable")
+        self._init_p = p
+        self.learn, self.channels = learn, channels
+        self.p = torch.nn.Parameter(torch.empty(channels)) if learn else p
+        self.reset_parameters()
+        self.min_value, self.max_value = clamp_min, clamp_max
+
+    def reset_parameters(self):
+        if isinstance(self.p, Tensor):
+            self.p.data.fill_(self._init_p)
+
+    def forward(self, x, index=None, ptr=None, dim_size=None, dim=-2, index_sorted=False):
+        d = dim + x.dim() if dim < 0 else dim
+        if self.channels != 1:                                           # base.py:162-169
+            if x.dim() != 2:
+                raise ValueError(f"Aggregation requires two-dimensional inputs (got '{x.dim()}')")
+            if dim not in (-2, 0):
+                raise ValueError(f"Aggregation needs to perform aggregation in first dimension (got '{dim}')")
+        if not power_mean_fusable(x, self.p, self.min_value, self.max_value):
+            return self._composed(x, index, ptr, dim_size, d, index_sorted)
+        xm = x.movedim(d, 0)
+        rest = xm.shape[1:]
+        x2 = xm.reshape(xm.size(0), -1)
+        out = _group_forward(Fn.power_mean_aggregate, x2, index, ptr, dim_size, index_sorted, p=self.p,
+                             clamp_min=self.min_value, clamp_max=self.max_value)
+        return out.view(out.size(0), *rest).movedim(0, d)
+
+    def _composed(self, x, index, ptr, dim_size, d, index_sorted):
+        """The reference's op sequence (basic.py:279-293) on the engine's mean: for messages the fused sweep does not
+        take (fp16, fp64), a p whose dtype differs from the messages' (x.pow(p) promotes, and the result takes the
+        promoted dtype), and clamp bounds off the fused path."""
+        p = self.p
+        if self.channels != 1:
+            p = p.view(-1, self.channels)
+        pow_ = not isinstance(p, (int, float)) or p != 1
+        if pow_:
+            x = x.clamp(min=self.min_value, max=self.max_value).pow(p)
+        out = self.reduce(x, index, ptr, dim_size, d, "mean", index_sorted)
+        if pow_:
+            out = out.clamp(min=self.min_value, max=self.max_value).pow(1. / p)
+        return out
+
+    def __repr__(self) -> str:
+        return f"{self.__class__.__name__}(learn={self.learn})"
+
+
+def power_mean_fusable(x: Tensor, p, clamp_min, clamp_max) -> bool:
+    """The fused sweep takes CUDA float32 / bfloat16 messages with a Python-number p or a p of the messages' dtype, and,
+    unless p is the number 1, a positive clamp_min with clamp_max None or >= clamp_min."""
+    if not (x.is_cuda and x.dtype in (torch.float32, torch.bfloat16)):
+        return False
+    if not isinstance(p, Tensor):
+        if float(p) == 1.0:
+            return True
+    elif p.dtype != x.dtype:
+        return False
+    return (isinstance(clamp_min, (int, float)) and clamp_min > 0 and
+            (clamp_max is None or (isinstance(clamp_max, (int, float)) and clamp_max >= clamp_min)))
+
+
+def _group_forward(fn, x, index, ptr, dim_size, index_sorted, **kw):
+    """fn(graph, None, x, **kw) over a [E, F] message matrix grouped by ptr or index (as _fused_forward groups them)."""
+    if ptr is None and index is None:
+        raise NotImplementedError("Aggregation requires 'index' to be specified")
+    if ptr is None and index_sorted:
+        ptr = ops.index2ptr(index, dim_size)
+    if ptr is not None:
+        return fn((ptr, ops.segment_plan(ptr, x.size(0))), None, x, **kw)
+    # unsorted index: a CSR over the messages themselves; the sweep reads message perm[e] of CSR slot e in place
+    from ..graph import CSRGraph
+    e = torch.arange(index.numel(), device=index.device, dtype=index.dtype)
+    return fn(CSRGraph(e, index, index.numel(), dim_size), None, x, **kw)
+
+
 class VarAggregation(Aggregation):
     """var = mean(x^2) - mean(x)^2 per group (nn/aggr/basic.py:83-111), one fused sweep."""
     fused_name = "var"
@@ -301,7 +384,8 @@ class MultiAggregation(Aggregation):
 
 def aggregation_resolver(name: str, **kwargs) -> Aggregation:
     table = {"sum": SumAggregation, "add": SumAggregation, "mean": MeanAggregation, "max": MaxAggregation,
-             "min": MinAggregation, "var": VarAggregation, "std": StdAggregation, "softmax": SoftmaxAggregation}
+             "min": MinAggregation, "var": VarAggregation, "std": StdAggregation, "softmax": SoftmaxAggregation,
+             "powermean": PowerMeanAggregation}
     if name not in table:
         raise ValueError(f"Could not resolve '{name}' among the aggregations on the hot path {sorted(table)}")
     return table[name](**kwargs)

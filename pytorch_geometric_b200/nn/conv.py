@@ -14,6 +14,7 @@ Two layers of code:
       GINEConv        nn/conv/gin_conv.py:104-207        nn.*, eps [1], lin.weight/bias (edge_dim)
       ResGatedGraphConv nn/conv/res_gated_graph_conv.py:13-148  lin_key/lin_query/lin_value.weight/bias, lin_skip.weight, bias
       CGConv          nn/conv/cg_conv.py:12-101          lin_f.weight/bias, lin_s.weight/bias, bn.* (batch_norm)
+      GENConv         nn/conv/gen_conv.py:45-243         aggr_module.t/p, lin_src/lin_edge/lin_dst.weight, mlp.*, msg_norm.scale
       PNAConv         nn/conv/pna_conv.py:20-209         aggr_module.avg_deg_lin/log, edge_encoder.*, pre_nns.t.0.*, post_nns.*, lin.*
       RGCNConv        nn/conv/rgcn_conv.py:40-300        weight [R,in,out] (or bases/blocks + comp), root, bias
       FastRGCNConv    nn/conv/rgcn_conv.py:302-374       same parameters
@@ -1053,3 +1054,94 @@ class HeteroLinear(torch.nn.Module):
     def __repr__(self) -> str:
         return (f"{self.__class__.__name__}({self.in_channels}, {self.out_channels}, num_types={self.num_types}, "
                 f"bias={self.bias is not None})")
+
+
+class _MessageNorm(torch.nn.Module):
+    """torch_geometric.nn.norm.MessageNorm (nn/norm/msg_norm.py:8-50): normalize(msg) * ||x|| * scale."""
+
+    def __init__(self, learn_scale: bool = False):
+        super().__init__()
+        self.scale = torch.nn.Parameter(torch.ones(1), requires_grad=learn_scale)
+
+    def reset_parameters(self):
+        self.scale.data.fill_(1.0)
+
+    def forward(self, x: Tensor, msg: Tensor) -> Tensor:
+        return F.normalize(msg, p=2.0, dim=-1) * x.norm(p=2.0, dim=-1, keepdim=True) * self.scale
+
+
+def _gen_mlp(channels, norm: Optional[str], bias: bool) -> torch.nn.Sequential:
+    """GENConv's MLP (gen_conv.py:21-42) for norm in {'batch', None}: Linear, [BatchNorm1d,] ReLU, Dropout(0) per hidden
+    layer, so that the state_dict keys are the reference's (mlp.0.weight, mlp.1.running_mean, ...)."""
+    m = []
+    for i in range(1, len(channels)):
+        m.append(_Lin(channels[i - 1], channels[i], bias=bias))
+        if i < len(channels) - 1:
+            if norm == "batch":
+                m.append(torch.nn.BatchNorm1d(channels[i], affine=True))
+            m.append(torch.nn.ReLU())
+            m.append(torch.nn.Dropout(0.0))
+    return torch.nn.Sequential(*m)
+
+
+class GENConv(torch.nn.Module):
+    """x_dst + MLP(AGGR_j (relu(x_j + e_ji) + eps)) (gen_conv.py:45-243) with AGGR the softmax aggregation (t, learn_t,
+    'softmax_sg') or the power mean (p, learn_p): the message and its aggregation run as one sweep
+    (`Fn.softmax_aggregate` / `Fn.power_mean_aggregate` with the relu_eps message), nothing stored per edge.  t and p
+    are read in fp32 on the device.  Other aggregations, and norms other than 'batch' and None, raise ValueError."""
+
+    AGGRS = ("softmax", "softmax_sg", "powermean", "power")
+
+    def __init__(self, in_channels, out_channels: int, aggr: str = "softmax", t: float = 1.0, learn_t: bool = False,
+                 p: float = 1.0, learn_p: bool = False, msg_norm: bool = False, learn_msg_scale: bool = False,
+                 norm: Optional[str] = "batch", num_layers: int = 2, expansion: int = 2, eps: float = 1e-7,
+                 bias: bool = False, edge_dim: Optional[int] = None, **kwargs):
+        super().__init__()
+        from .aggr import PowerMeanAggregation, SoftmaxAggregation
+        if not isinstance(aggr, str) or aggr not in self.AGGRS:
+            raise ValueError(f"aggr={aggr!r} is not on the fused path (supported: {self.AGGRS})")
+        if norm not in ("batch", None):
+            raise ValueError(f"norm={norm!r} is not supported (supported: 'batch', None)")
+        semi_grad = aggr == "softmax_sg"
+        self.aggr = "softmax" if aggr in ("softmax", "softmax_sg") else "powermean"   # gen_conv.py:141-143
+        akw = kwargs.pop("aggr_kwargs", None)
+        if akw is None:
+            akw = dict(t=t, learn=learn_t, semi_grad=semi_grad) if self.aggr == "softmax" else dict(p=p, learn=learn_p)
+        self.aggr_module = SoftmaxAggregation(**akw) if self.aggr == "softmax" else PowerMeanAggregation(**akw)
+        self.flow = kwargs.pop("flow", "source_to_target")
+        self.in_channels, self.out_channels, self.eps = in_channels, out_channels, eps
+        ch = (in_channels, in_channels) if isinstance(in_channels, int) else tuple(in_channels)
+        if ch[0] != out_channels:
+            self.lin_src = _Lin(ch[0], out_channels, bias=bias)
+        if edge_dim is not None and edge_dim != out_channels:
+            self.lin_edge = _Lin(edge_dim, out_channels, bias=bias)
+        if ch[1] != out_channels:
+            self.lin_dst = _Lin(ch[1], out_channels, bias=bias)
+        self.mlp = _gen_mlp([out_channels] + [out_channels * expansion] * (num_layers - 1) + [out_channels], norm, bias)
+        if msg_norm:
+            self.msg_norm = _MessageNorm(learn_msg_scale)
+
+    def forward(self, x, edge_index: Adj, edge_attr: Optional[Tensor] = None, size=None) -> Tensor:
+        from .aggr import SoftmaxAggregation
+        pair = _pair(x)
+        x_src = self.lin_src(pair[0]) if hasattr(self, "lin_src") else pair[0]
+        n_dst = pair[1].size(0) if pair[1] is not None else (size[1] if size is not None else x_src.size(0))
+        graph = _plain_graph(edge_index, x_src.size(0), n_dst, self.flow)
+        ea = edge_attr
+        if ea is not None and hasattr(self, "lin_edge"):
+            ea = self.lin_edge(ea)
+        if ea is not None and ea.size(-1) != x_src.size(-1):
+            raise ValueError(f"edge features have {ea.size(-1)} channels, the messages {x_src.size(-1)}")
+        a = self.aggr_module
+        if isinstance(a, SoftmaxAggregation):
+            out = Fn.softmax_aggregate(graph, x_src, ea, a.t, self.eps, "relu_eps", a.semi_grad and not a.learn)
+        else:
+            out = Fn.power_mean_aggregate(graph, x_src, ea, a.p, self.eps, "relu_eps", a.min_value, a.max_value)
+        if hasattr(self, "msg_norm"):                                             # gen_conv.py:218-221
+            out = self.msg_norm(pair[1] if pair[1] is not None else x_src, out)
+        if pair[1] is not None:
+            out = out + (self.lin_dst(pair[1]) if hasattr(self, "lin_dst") else pair[1])
+        return self.mlp(out)
+
+    def __repr__(self) -> str:
+        return f"{self.__class__.__name__}({self.in_channels}, {self.out_channels}, aggr={self.aggr})"

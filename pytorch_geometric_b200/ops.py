@@ -669,6 +669,95 @@ def softmax_aggr_backward_src(rowptr_t: Tensor, col_t: Tensor, perm_t: Tensor, x
     return grad_x
 
 
+def _power_mean_args(x: Optional[Tensor], a: Optional[Tensor], p: Optional[Tensor], message: str, n_edges: int,
+                     clamp_min: float, clamp_max: Optional[float]):
+    """Check the operands of the power-mean sweeps; returns (F, message code, p_mode, lo, hi).  As
+    _softmax_aggr_args, with p: None (a plain mean) or fp32 [1] / [F]; with p, clamp_min > 0 and clamp_max None
+    (no upper bound) or >= clamp_min."""
+    F, msg, p_mode = _softmax_aggr_args(x, a, p, message, n_edges)
+    hi = float("inf") if clamp_max is None else float(clamp_max)
+    lo = 0.0 if clamp_min is None else float(clamp_min)
+    if p is not None and not (lo > 0.0 and hi >= lo):
+        raise ValueError(f"the power-mean sweep needs 0 < clamp_min <= clamp_max, got {clamp_min} and {clamp_max}")
+    return F, msg, p_mode, lo, hi
+
+
+def power_mean_csr(rowptr: Tensor, col: Optional[Tensor], perm: Optional[Tensor], x: Optional[Tensor],
+                   a: Optional[Tensor], p: Optional[Tensor], n_rows: int, n_edges: int, message: str = "identity",
+                   eps: float = 0.0, clamp_min: float = 1e-4, clamp_max: Optional[float] = 100.0,
+                   plan: Optional[LongRowPlan] = None, want_mean: bool = False) -> Tuple[Tensor, Optional[Tensor]]:
+    """out[i] = clamp(mean_e clamp(m_e)^p)^(1/p) over row i (b200mp_power_mean_csr), m_e as in softmax_aggr_csr; p None
+    is a plain mean.  With want_mean also the fp32 plane of the means M the backward reads."""
+    _cuda(rowptr, col, perm, x, a, p)
+    F, msg, p_mode, lo, hi = _power_mean_args(x, a, p, message, n_edges, clamp_min, clamp_max)
+    it = _same_idx(rowptr, col, perm)
+    ref = x if x is not None else a
+    out = torch.empty(n_rows, F, dtype=ref.dtype, device=ref.device)
+    mean = torch.empty(n_rows, F, dtype=torch.float32, device=ref.device) if want_mean else None
+    pargs, _ = _plan_args(plan, F, ref.device)
+    _timed("power_mean_csr", 2 if pargs[2] else 1, lib().b200mp_power_mean_csr, _p(rowptr), _p(col), _p(perm), _p(x),
+           _p(a), _p(p), _p(out), _p(mean), n_rows, 0 if x is None else x.size(0), n_edges, F, msg, float(eps), p_mode,
+           lo, hi, *pargs, it, _vdt(ref), _stream())
+    return out, mean
+
+
+def power_mean_backward_dst(rowptr: Tensor, col: Optional[Tensor], perm: Optional[Tensor], x: Optional[Tensor],
+                            a: Optional[Tensor], p: Optional[Tensor], out: Tensor, mean: Optional[Tensor],
+                            grad_out: Tensor, n_edges: int, message: str, eps: float, clamp_min: float,
+                            clamp_max: Optional[float], want_grad_a: bool, want_grad_p: bool,
+                            plan: Optional[LongRowPlan] = None):
+    """Destination sweep of the power-mean backward: (grad_a [E, F] in the caller's edge order or None, grad_p [F]
+    fp32 per-channel sums or None)."""
+    _cuda(rowptr, col, perm, x, a, p, out, mean, grad_out)
+    F, msg, p_mode, lo, hi = _power_mean_args(x, a, p, message, n_edges, clamp_min, clamp_max)
+    if want_grad_p and p is None:
+        raise ValueError("grad_p needs p")
+    it = _same_idx(rowptr, col, perm)
+    grad_out = grad_out.contiguous()
+    n_rows = rowptr.numel() - 1
+    grad_a = torch.empty(n_edges, F, dtype=out.dtype, device=out.device) if want_grad_a else None
+    grad_p = ws = None
+    n_chunks = plan.n_chunks if plan is not None and plan.n_long else 0
+    if want_grad_p:
+        grad_p = torch.empty(F, dtype=torch.float32, device=out.device)
+        ws = torch.empty(max(int(lib().b200mp_power_mean_workspace(0, n_rows, n_chunks, F)), 1), dtype=torch.float32,
+                         device=out.device)
+    # the destination sweep only splits long rows (nothing to combine): the plan without partials
+    pargs = _plan_args(None, F, out.device)[0] if not n_chunks else (_p(plan.long_rows), _p(plan.chunk_ptr), plan.n_long,
+                                                                     plan.n_chunks, plan.chunk)
+    _timed("power_mean_backward_dst", 3 if want_grad_p else 1, lib().b200mp_power_mean_backward_dst, _p(rowptr),
+           _p(col), _p(perm), _p(x), _p(a), _p(p), _p(out), _p(mean), _p(grad_out), _p(grad_a), _p(grad_p), _p(ws),
+           n_rows, 0 if x is None else x.size(0), n_edges, F, msg, float(eps), p_mode, lo, hi, *pargs[:5], it,
+           _vdt(out), _stream())
+    return grad_a, grad_p
+
+
+def power_mean_backward_src(rowptr: Tensor, rowptr_t: Tensor, col_t: Tensor, perm_t: Tensor, x: Tensor,
+                            a: Optional[Tensor], p: Optional[Tensor], out: Tensor, mean: Optional[Tensor],
+                            grad_out: Tensor, message: str, eps: float, clamp_min: float, clamp_max: Optional[float],
+                            want_grad_p: bool, plan_t: Optional[LongRowPlan] = None):
+    """Node kernel and transposed-CSR sweep of the power-mean backward: (grad_x [n_src, F] (a frozen), grad_p [F] fp32
+    per-channel sums or None).  rowptr: the destination CSR's, for the degrees."""
+    _cuda(rowptr, rowptr_t, col_t, perm_t, x, a, p, out, mean, grad_out)
+    E = col_t.numel()
+    F, msg, p_mode, lo, hi = _power_mean_args(x, a, p, message, E, clamp_min, clamp_max)
+    if want_grad_p and p is None:
+        raise ValueError("grad_p needs p")
+    it = _same_idx(rowptr, rowptr_t, col_t, perm_t)
+    grad_out = grad_out.contiguous()
+    grad_x = torch.empty_like(x)
+    n_dst = out.size(0)
+    grad_p = torch.empty(F, dtype=torch.float32, device=x.device) if want_grad_p else None
+    pargs, _ = _plan_args(plan_t, F, x.device)
+    ws = torch.empty(max(int(lib().b200mp_power_mean_workspace(n_dst, x.size(0), pargs[3], F)), 1),
+                     dtype=torch.float32, device=x.device)
+    _timed("power_mean_backward_src", (2 if pargs[2] else 1) + (3 if want_grad_p else 1),
+           lib().b200mp_power_mean_backward_src, _p(rowptr), _p(rowptr_t), _p(col_t), _p(perm_t), _p(x), _p(a), _p(p),
+           _p(out), _p(mean), _p(grad_out), _p(grad_x), _p(grad_p), _p(ws), x.size(0), n_dst, E, F, msg, float(eps),
+           p_mode, lo, hi, *pargs, it, _vdt(x), _stream())
+    return grad_x, grad_p
+
+
 def scatter_coo(src: Tensor, index: Tensor, n_rows: int, reduce: str = "sum") -> Tensor:
     """Atomic COO fallback for an unsorted index; fp32, src: [E, F]."""
     _cuda(src, index)

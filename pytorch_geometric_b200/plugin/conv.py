@@ -36,7 +36,7 @@ from ._util import plain
 # Inspector caches class sources by `cls.__name__` (torch_geometric/inspector.py:323-334), so a subclass that reused
 # its parent's name would hide the parent's `# propagate_type:` annotation and get a `propagate` without arguments.
 LAYERS = {n: "B200" + n for n in ("GCNConv", "SAGEConv", "GraphConv", "GINConv", "GATConv", "GATv2Conv", "TransformerConv",
-                                  "RGCNConv", "FastRGCNConv", "PNAConv", "CGConv")}
+                                  "RGCNConv", "FastRGCNConv", "PNAConv", "CGConv", "GENConv")}
 
 
 def _has_hooks(self) -> bool:
@@ -348,3 +348,61 @@ class B200CGConv(tgnn.CGConv):
                 out = out if self.bn is None else self.bn(out)                       # cg_conv.py:86-88
                 return out + xs[1]
         return super().forward(x, edge_index, edge_attr)
+
+
+def _gen_fusable(self, xs, edge_index, edge_attr) -> bool:
+    """The fused GENConv path covers the reference's SoftmaxAggregation (t, learn_t, softmax_sg, channels) and
+    PowerMeanAggregation (p, learn_p, channels, clamp bounds the sweep takes) without lin_aggr_out, a [2, E] tensor or
+    EdgeIndex adjacency, and CUDA float32 / bfloat16 inputs of one dtype whose t or p is a number or of that dtype (a
+    learnable fp32 t or p with bf16 inputs promotes in the reference: it stays there)."""
+    aggr = self.aggr_module
+    if type(aggr) is tgnn.aggr.SoftmaxAggregation:
+        w = aggr.t
+    elif type(aggr) is tgnn.aggr.PowerMeanAggregation:
+        w = aggr.p
+    else:
+        return False
+    if hasattr(self, "lin_aggr_out") or xs[0] is None or xs[0].dim() != 2:
+        return False
+    if not (isinstance(edge_index, Tensor) and edge_index.layout == torch.strided and edge_index.dim() == 2
+            and edge_index.size(0) == 2 and not edge_index.is_floating_point()):
+        return False
+    if edge_attr is not None and edge_attr.dim() != 2:
+        return False
+    ts = [t for t in (xs[0], xs[1], edge_attr) if t is not None]
+    if not _fast(self, *ts) or len({t.dtype for t in ts}) != 1:
+        return False
+    if isinstance(w, Tensor) and (w.dtype != xs[0].dtype or w.numel() not in (1, self.out_channels)):
+        return False
+    if type(aggr) is tgnn.aggr.PowerMeanAggregation:
+        from ..nn.aggr import power_mean_fusable
+        return power_mean_fusable(xs[0], w, aggr.min_value, aggr.max_value)
+    return True
+
+
+class B200GENConv(tgnn.GENConv):
+    def forward(self, x, edge_index, edge_attr=None, size=None) -> Tensor:
+        xs = _pair(x)
+        if _gen_fusable(self, xs, edge_index, edge_attr):
+            g = _graph(edge_index, xs[0].size(0), _ndst(xs, size), self.flow)
+            if g is not None:
+                x_src = self.lin_src(xs[0]) if hasattr(self, "lin_src") else xs[0]            # gen_conv.py:209-210
+                ea = edge_attr
+                if ea is not None and hasattr(self, "lin_edge"):                              # gen_conv.py:232-233
+                    ea = self.lin_edge(ea)
+                aggr = self.aggr_module
+                if type(aggr) is tgnn.aggr.SoftmaxAggregation:
+                    out = Fn.softmax_aggregate(g, x_src, ea, aggr.t, self.eps, "relu_eps",
+                                               aggr.semi_grad and not aggr.learn)
+                else:
+                    out = Fn.power_mean_aggregate(g, x_src, ea, aggr.p, self.eps, "relu_eps", aggr.min_value,
+                                                  aggr.max_value)
+                if hasattr(self, "msg_norm"):                                                 # gen_conv.py:218-221
+                    out = self.msg_norm(xs[1] if xs[1] is not None else x_src, out)
+                x_dst = xs[1]
+                if x_dst is not None:
+                    if hasattr(self, "lin_dst"):
+                        x_dst = self.lin_dst(x_dst)
+                    out = out + x_dst
+                return self.mlp(out)
+        return super().forward(x, edge_index, edge_attr, size)

@@ -337,7 +337,8 @@ int64_t b200mp_softmax_aggr_workspace(int64_t n_rows, int64_t n_chunks, int64_t 
  *   grad_m_e = g p_e (1 + t (m_e - o))   (semi_grad: g p_e)        grad_s_e = grad_m_e [s_e > 0 or NaN] (message 1)
  *   grad_edge_rows[eid(e)] = grad_s_e  (NULL: not written)          grad_t[f] = sum_i sum_e g p_e m_e (m_e - o)
  * grad_t: NULL or [feat] fp32 (per-channel sums; the caller sums them for a scalar t), from per-CTA partials folded
- * in fixed order by b200mp_column_sum in `workspace` (b200mp_softmax_aggr_workspace elements).  The 1e-16 of the
+ * in fixed order by b200mp_column_sum in `workspace` (b200mp_softmax_aggr_workspace elements).  With grad_t, the
+ * feat limit of b200mp_power_mean_backward_dst's grad_p applies (B200MP_ERR_UNSUPPORTED beyond it).  The 1e-16 of the
  * forward's denominator is dropped here: the denominator is >= 1, so it is below fp32 resolution. */
 int b200mp_softmax_aggr_backward_dst(const void* rowptr, const void* col, const void* perm, const void* x,
                                      const void* edge_rows, const float* t, const void* out, const float* lse,
@@ -376,13 +377,13 @@ int b200mp_softmax_aggr_backward_src(const void* rowptr_t, const void* col_t, co
 int b200mp_power_mean_csr(const void* rowptr, const void* col, const void* perm, const void* x,
                           const void* edge_rows, const float* p, void* out, float* mean, int64_t n_rows,
                           int64_t n_cols, int64_t n_edges, int64_t feat, int message, float eps, int p_mode,
-                          float clamp_min, float clamp_max, const int64_t* plan_long_rows, const int64_t* plan_chunk_ptr,
-                          int64_t plan_n_long_rows, int64_t plan_n_chunks, int64_t plan_chunk, float* plan_partials, int idx_dtype,
+                          float clamp_min, float clamp_max, const int64_t* long_rows, const int64_t* chunk_ptr,
+                          int64_t n_long_rows, int64_t n_chunks, int64_t chunk, float* partials, int idx_dtype,
                           int val_dtype, void* stream);
 /* fp32 workspace elements of the power-mean backward: b200mp_power_mean_backward_dst over n_rows destination rows
  * (n_node = 0), or b200mp_power_mean_backward_src over n_rows source rows of the transposed CSR with n_node = n_dst
  * (its node plane). */
-int64_t b200mp_power_mean_workspace(int64_t n_node, int64_t n_rows, int64_t plan_n_chunks, int64_t feat);
+int64_t b200mp_power_mean_workspace(int64_t n_node, int64_t n_rows, int64_t n_chunks, int64_t feat);
 /* Destination sweep of the backward (replaces the autograd of basic.py:275-293 / gen_conv.py:231-239 over [E, F]).
  * Recomputes m, c and y; with g = grad_out[i], o = out[i] and C_i = clamp(M_i):
  *   G_i = g (1/p) C_i ^ (1/p - 1) / max(deg_i, 1) [clamp_min <= M_i <= clamp_max]   (p_mode 0: g / max(deg_i, 1))
@@ -390,27 +391,30 @@ int64_t b200mp_power_mean_workspace(int64_t n_node, int64_t n_rows, int64_t plan
  *   grad_edge_rows[eid(e)] = grad_s_e (NULL: not written)
  *   grad_p[f] = sum_i sum_e G_i y_e ln c_e - sum_i g o ln C_i / p^2     (the second sum includes empty rows)
  * grad_p: NULL or [feat] fp32 (per-channel sums; the caller sums them for a scalar p), from per-CTA partials folded in
- * fixed order by b200mp_column_sum in `workspace` (b200mp_power_mean_workspace(0, n_rows, plan_n_chunks, feat)). */
+ * fixed order by b200mp_column_sum in `workspace` (b200mp_power_mean_workspace(0, n_rows, n_chunks, feat)).  With
+ * grad_p, feat is at most about 7,000 on the scalar path and 14,000 on the 16-byte vector path: wider rows return
+ * B200MP_ERR_UNSUPPORTED before anything is launched, because each lane group keeps one fp32 row of grad_p partials
+ * in shared memory.  b200mp_power_mean_backward_src has the same limit. */
 int b200mp_power_mean_backward_dst(const void* rowptr, const void* col, const void* perm, const void* x,
                                    const void* edge_rows, const float* p, const void* out, const float* mean,
                                    const void* grad_out, void* grad_edge_rows, float* grad_p, float* workspace,
                                    int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t feat, int message,
-                                   float eps, int p_mode, float clamp_min, float clamp_max, const int64_t* plan_long_rows,
-                                   const int64_t* plan_chunk_ptr, int64_t plan_n_long_rows, int64_t plan_n_chunks, int64_t plan_chunk,
+                                   float eps, int p_mode, float clamp_min, float clamp_max, const int64_t* long_rows,
+                                   const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks, int64_t chunk,
                                    int idx_dtype, int val_dtype, void* stream);
 /* grad_x (and grad_p) by ONE sweep over the TRANSPOSED CSR: a node kernel first writes G_i of every destination into
- * `workspace` (b200mp_power_mean_workspace(n_dst, n_src, plan_n_chunks, feat)) with the per-row grad_p terms, then
+ * `workspace` (b200mp_power_mean_workspace(n_dst, n_src, n_chunks, feat)) with the per-row grad_p terms, then
  * grad_x[j] = sum_{t in rowT(j)} grad_s_t gathers one fp32 row of G at col_t[t] and edge_rows[perm_t[t]] (frozen edge
  * rows) per out-edge.  rowptr: the destination CSR's (for the degrees).  Needs x.  Used when no grad_edge_rows was
  * written; otherwise the segment sum of grad_edge_rows over the transposed CSR (b200mp_spmm_csr with perm_t as the
- * column) gives grad_x with fewer bytes.  Long source rows: the transposed CSR's plan, partials [plan_n_chunks, feat]. */
+ * column) gives grad_x with fewer bytes.  Long source rows: the transposed CSR's plan, partials [n_chunks, feat]. */
 int b200mp_power_mean_backward_src(const void* rowptr, const void* rowptr_t, const void* col_t, const void* perm_t,
                                    const void* x, const void* edge_rows, const float* p, const void* out,
                                    const float* mean, const void* grad_out, void* grad_x, float* grad_p,
                                    float* workspace, int64_t n_src, int64_t n_dst, int64_t n_edges, int64_t feat,
                                    int message, float eps, int p_mode, float clamp_min, float clamp_max,
-                                   const int64_t* plan_long_rows, const int64_t* plan_chunk_ptr, int64_t plan_n_long_rows,
-                                   int64_t plan_n_chunks, int64_t plan_chunk, float* plan_partials, int idx_dtype, int val_dtype,
+                                   const int64_t* long_rows, const int64_t* chunk_ptr, int64_t n_long_rows,
+                                   int64_t n_chunks, int64_t chunk, float* partials, int idx_dtype, int val_dtype,
                                    void* stream);
 
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)

@@ -79,6 +79,13 @@ void lane_group_shape(int n_vec, F&& launch) {
     else launch(integral_constant<int, 32>{}, integral_constant<int, 4>{});
 }
 
+// log2 of lane_group_shape's G, for kernels that take the group width at run time.
+inline int lane_group_log2(int n_vec) {
+    int lg = 0;
+    lane_group_shape<1>(n_vec, [&](auto G, auto) { lg = __builtin_ctz(decltype(G)::value); });
+    return lg;
+}
+
 // Independent edges in flight per lane for VPL vectors per lane: about 4 sixteen-byte row loads.
 template <int VPL>
 constexpr int unroll_for_vpl() { return VPL >= 4 ? 1 : 4 / VPL; }

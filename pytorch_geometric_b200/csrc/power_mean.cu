@@ -30,36 +30,11 @@
 // Mapping as in softmax_aggr.cu: a lane group of G lanes per row, one 16-byte vector per lane and trip, rows longer
 // than the plan's chunk split into chunks whose fp32 partials a combine kernel folds in chunk order.  Rows that are not
 // a whole number of aligned 16-byte vectors take a one-warp scalar kernel.
-#include "aggr_message.cuh"
-#include "csr_reduce.cuh"
-
-extern "C" int b200mp_column_sum(const void* x, float* out, float* partials, int64_t n_parts, int64_t n_rows,
-                                 int64_t feat, int val_dtype, void* stream);
-extern "C" int64_t b200mp_column_sum_parts(int64_t n_rows);
+#include "param_aggr.cuh"
 
 namespace b200mp {
 
-enum PmMode { kPmFwd = 0, kPmDst = 1, kPmSrc = 2 };
-enum PmP { kPmPNone = 0, kPmPScalar = 1, kPmPChannel = 2 };
-
 constexpr int kPmNodeRows = 32;   // destination rows per CTA of the node kernel
-// The grad_p sweeps keep one fp32 row of F per lane group in shared memory: H100's opt-in limit per CTA.
-constexpr size_t kPmMaxSmem = 227 * 1024;
-
-struct PmArgs {
-    const void* x;       // [n_src, feat] gathered through col (fwd / dst) or the row operand (src)
-    const void* a;       // [n_edges, feat] in the caller's edge order
-    const float* p;      // [1] or [feat] fp32
-    const void* perm;    // caller's edge id of each CSR (fwd / dst) or transposed (src) slot; null = slot
-    const void* g;       // grad_out [n_dst, feat]
-    const void* o;       // out [n_dst, feat]
-    float* M;            // [n_dst, feat]: written by fwd (nullable), read by the backward
-    float* G;            // src: the node plane [n_dst, feat] the transposed sweep gathers
-    void* out;           // fwd: out; dst: grad_a (nullable); src: grad_x
-    float* gp_part;      // [gridDim.x, feat] grad_p partials, or null
-    int64_t feat;
-    float eps, lo, hi;
-};
 
 // clamp(v, lo, hi) keeping NaN (fminf / fmaxf would drop it).
 __device__ __forceinline__ float pm_clamp(float v, float lo, float hi) {
@@ -86,14 +61,14 @@ __device__ __forceinline__ float pm_pow(float c, float p) {
 // y = round(clamp(m) ^ p), or m without p.
 template <typename T, int PMODE>
 __device__ __forceinline__ float pm_term(float m, float p, float lo, float hi) {
-    return PMODE == kPmPNone ? m : round_to<T>(pm_pow(pm_clamp(m, lo, hi), p));
+    return PMODE == kParamNone ? m : round_to<T>(pm_pow(pm_clamp(m, lo, hi), p));
 }
 
 // out from the fp32 sum of a row's terms; M is the saved (rounded) mean.
 template <typename T, int PMODE>
 __device__ __forceinline__ float pm_final(float S, float d, float p, float lo, float hi, float& M) {
     M = round_to<T>(__fdiv_rn(S, d));
-    return PMODE == kPmPNone ? M : round_to<T>(pm_pow(pm_clamp(M, lo, hi), __frcp_rn(p)));
+    return PMODE == kParamNone ? M : round_to<T>(pm_pow(pm_clamp(M, lo, hi), __frcp_rn(p)));
 }
 
 // G_i of a destination element: g (1/p) C ^ (1/p - 1) / deg under the clamp mask, as ATen's pow backward forms it (so
@@ -101,7 +76,7 @@ __device__ __forceinline__ float pm_final(float S, float d, float p, float lo, f
 // backward divides with __fdividef (2 ulp): an IEEE division's slow-path call would cost the sweeps a stack frame.
 template <int PMODE, bool WANT_P>
 __device__ __forceinline__ float pm_node(float g, float o, float M, float d, float p, float lo, float hi, float& gp) {
-    if (PMODE == kPmPNone) return __fdividef(g, d);
+    if (PMODE == kParamNone) return __fdividef(g, d);
     const float C = pm_clamp(M, lo, hi);
     const float lC = pm_lg2(C);
     const float rp = __frcp_rn(p);
@@ -114,7 +89,7 @@ __device__ __forceinline__ float pm_node(float g, float o, float M, float d, flo
 // WANT_P.
 template <int PMODE, bool WANT_P>
 __device__ __forceinline__ float pm_grad(float m, float G, float p, float lo, float hi, float& gp) {
-    if (PMODE == kPmPNone) return G;
+    if (PMODE == kParamNone) return G;
     const float c = pm_clamp(m, lo, hi);
     const float l = pm_lg2(c);
     if (WANT_P) gp = fmaf(__fmul_rn(G, pm_ex2(__fmul_rn(p, l))), __fmul_rn(l, 0.69314718055994531f), gp);
@@ -131,11 +106,6 @@ __device__ __forceinline__ void pm_kahan(float& s, float& c, float v) {
     s = t;
 }
 
-template <typename I>
-__device__ __forceinline__ int64_t pm_eid(const PmArgs& a, int64_t e) {
-    return a.perm ? static_cast<int64_t>(ldg_idx(static_cast<const I*>(a.perm) + e)) : e;
-}
-
 // max(deg, 1) of a row as fp32: the divisor of the mean.
 template <typename I>
 __device__ __forceinline__ float pm_deg(const I* rowptr, int64_t row) {
@@ -143,44 +113,33 @@ __device__ __forceinline__ float pm_deg(const I* rowptr, int64_t row) {
     return static_cast<float>(d < 1 ? 1 : d);
 }
 
-// Per-CTA grad_p partial: every group has written its row of `sh` (zeros when idle); fold the groups in order.
-__device__ __forceinline__ void pm_store_gp(const float* sh, int groups, int64_t feat, float* gp_part) {
-    __syncthreads();
-    for (int64_t f = threadIdx.x; f < feat; f += blockDim.x) {
-        float s = 0.0f;
-        for (int k = 0; k < groups; ++k) s = __fadd_rn(s, sh[k * feat + f]);
-        gp_part[static_cast<int64_t>(blockIdx.x) * feat + f] = s;
-    }
-}
-
 // ---------------------------------------------------------------- the three sweeps, 16-byte vector path
 template <typename T, typename I, int MODE, int FORM, int PMODE, bool WANT_P>
 __global__ void __launch_bounds__(128, 1)
-power_mean_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, PmArgs args, int64_t n_rows, int n_vec,
+power_mean_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, AggrArgs args, int64_t n_rows, int n_vec,
                   int lg, LongRowPlan plan) {
     using Fm = SmForms<FORM>;
     constexpr int EPV = ElemTraits<T>::kPerVec;
-    constexpr int UNR = (MODE == kPmFwd || sizeof(T) == 4) ? 4 : 2;
+    constexpr int UNR = (MODE == kSweepFwd || sizeof(T) == 4) ? 4 : 2;
     extern __shared__ float pm_sh[];
     const int G = 1 << lg;
     const int lig = threadIdx.x & (G - 1);
     const int64_t item = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> lg;
     int64_t row = 0, begin = 0, end = 0;
     bool is_chunk = false;
-    const bool active = decode_item(item, rowptr, n_rows, plan, row, begin, end, is_chunk);   // uniform per group
+    const bool active = aggr_item<WANT_P>(item, rowptr, n_rows, plan, row, begin, end, is_chunk);   // uniform per group
     if (!active && !WANT_P) return;
-    if (!active) row = begin = end = 0;                  // an idle group still writes its (zero) grad_p row
     // the destination sweep adds a row's grad_p term once: in its whole-row item or its first chunk
     const bool row_term = active && (!is_chunk || begin == static_cast<int64_t>(ldg_idx(rowptr + row)));
     const float deg = active ? pm_deg(rowptr, row) : 1.0f;
     const int64_t F = args.feat;
     const size_t row_bytes = static_cast<size_t>(n_vec) * 16;
     const size_t row_off = static_cast<size_t>(row) * row_bytes;     // this row's byte offset in g, o, x (src) and out
-    const float* Mrow = args.M + static_cast<size_t>(row) * F;
+    const float* Mrow = args.saved + static_cast<size_t>(row) * F;
     const char* xb = static_cast<const char*>(args.x);
     const char* ab = static_cast<const char*>(args.a);
     float ps = 1.0f;
-    if (PMODE == kPmPScalar) ps = __ldg(args.p);
+    if (PMODE == kParamScalar) ps = __ldg(args.param);
 
 #pragma unroll 1
     for (int vi = lig; vi < n_vec; vi += G) {
@@ -189,14 +148,8 @@ power_mean_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, PmArg
         float pv[EPV], rx[EPV], rG[EPV], acc[EPV], cc[EPV], gp[EPV];
 #pragma unroll
         for (int i = 0; i < EPV; ++i) pv[i] = ps, rx[i] = rG[i] = acc[i] = cc[i] = gp[i] = 0.0f;
-        if (PMODE == kPmPChannel) {
-#pragma unroll
-            for (int i = 0; i < EPV; i += 4) {
-                const float4 p4 = __ldg(reinterpret_cast<const float4*>(args.p + f0 + i));
-                pv[i] = p4.x; pv[i + 1] = p4.y; pv[i + 2] = p4.z; pv[i + 3] = p4.w;
-            }
-        }
-        if (MODE == kPmDst && active) {
+        if (PMODE == kParamChannel) ldg_f32(args.param + f0, pv);
+        if (MODE == kSweepDst && active) {
             float rg[EPV], ro[EPV];
             ElemTraits<T>::unpack(ldg_stream16(static_cast<const char*>(args.g) + row_off + voff), rg);
             ElemTraits<T>::unpack(ldg_stream16(static_cast<const char*>(args.o) + row_off + voff), ro);
@@ -213,7 +166,7 @@ power_mean_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, PmArg
                 for (int q = 0; q < 4; ++q) gp[i + q] = row_term ? t[q] : 0.0f;
             }
         }
-        if (MODE == kPmSrc) ElemTraits<T>::unpack(ldg_stream16(xb + row_off + voff), rx);
+        if (MODE == kSweepSrc) ElemTraits<T>::unpack(ldg_stream16(xb + row_off + voff), rx);
         for (int64_t e = begin; e < end; e += UNR) {
             Vec16 xv[UNR], av[UNR];
             float4 gv[UNR][EPV / 4];
@@ -223,10 +176,10 @@ power_mean_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, PmArg
                 id[u] = 0;
                 if (e + u < end) {
                     const int64_t c = static_cast<int64_t>(ldg_idx(col + e + u));
-                    if (Fm::kA || (MODE == kPmDst && args.out)) id[u] = pm_eid<I>(args, e + u);
-                    if (MODE != kPmSrc && Fm::kX) xv[u] = ldg_row16(xb + c * row_bytes + voff);
+                    if (Fm::kA || (MODE == kSweepDst && args.out)) id[u] = aggr_eid<I>(args, e + u);
+                    if (MODE != kSweepSrc && Fm::kX) xv[u] = ldg_row16(xb + c * row_bytes + voff);
                     if (Fm::kA) av[u] = ldg_stream16(ab + id[u] * row_bytes + voff);
-                    if (MODE == kPmSrc) {
+                    if (MODE == kSweepSrc) {
                         const float4* gp4 = reinterpret_cast<const float4*>(args.G + c * F + f0);
 #pragma unroll
                         for (int q = 0; q < EPV / 4; ++q) gv[u][q] = __ldg(gp4 + q);
@@ -237,7 +190,7 @@ power_mean_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, PmArg
             for (int u = 0; u < UNR; ++u) {
                 if (e + u < end) {
                     float fx[EPV], fa[EPV], fG[EPV], gs[EPV];
-                    if (MODE == kPmSrc) {
+                    if (MODE == kSweepSrc) {
 #pragma unroll
                         for (int i = 0; i < EPV; ++i) fx[i] = rx[i];
 #pragma unroll
@@ -253,17 +206,17 @@ power_mean_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, PmArg
                     for (int i = 0; i < EPV; ++i) {
                         bool on;
                         const float m = sm_message<T, FORM>(fx[i], Fm::kA ? fa[i] : 0.0f, args.eps, on);
-                        if (MODE == kPmFwd) {
+                        if (MODE == kSweepFwd) {
                             pm_kahan(acc[i], cc[i], pm_term<T, PMODE>(m, pv[i], args.lo, args.hi));
                         } else {
-                            float gm = pm_grad<PMODE, WANT_P>(m, MODE == kPmSrc ? fG[i] : rG[i], pv[i], args.lo,
+                            float gm = pm_grad<PMODE, WANT_P>(m, MODE == kSweepSrc ? fG[i] : rG[i], pv[i], args.lo,
                                                               args.hi, gp[i]);
                             if (Fm::kRelu && !on) gm = 0.0f;
-                            if (MODE == kPmDst) gs[i] = gm;
+                            if (MODE == kSweepDst) gs[i] = gm;
                             else acc[i] = __fadd_rn(acc[i], gm);
                         }
                     }
-                    if (MODE == kPmDst && args.out)
+                    if (MODE == kSweepDst && args.out)
                         stg_stream16(static_cast<char*>(args.out) + id[u] * row_bytes + voff, ElemTraits<T>::pack(gs));
                 }
             }
@@ -273,8 +226,8 @@ power_mean_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, PmArg
 #pragma unroll
             for (int i = 0; i < EPV; ++i) sh[i] = gp[i];
         }
-        if (MODE == kPmDst || !active) continue;
-        if (MODE == kPmFwd) {
+        if (MODE == kSweepDst || !active) continue;
+        if (MODE == kSweepFwd) {
 #pragma unroll
             for (int i = 0; i < EPV; ++i) acc[i] = __fsub_rn(acc[i], cc[i]);
         }
@@ -283,23 +236,23 @@ power_mean_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, PmArg
             continue;
         }
         char* dst = static_cast<char*>(args.out) + row_off + voff;
-        if (MODE == kPmFwd) {
+        if (MODE == kSweepFwd) {
             float f[EPV], Mv[EPV];
 #pragma unroll
             for (int i = 0; i < EPV; ++i) f[i] = pm_final<T, PMODE>(acc[i], deg, pv[i], args.lo, args.hi, Mv[i]);
             stg_stream16(dst, ElemTraits<T>::pack(f));
-            if (args.M) store_partial<EPV>(args.M + static_cast<size_t>(row) * F + f0, Mv);
+            if (args.saved) store_partial<EPV>(args.saved + static_cast<size_t>(row) * F + f0, Mv);
         } else {
             stg_stream16(dst, ElemTraits<T>::pack(acc));
         }
     }
-    if (WANT_P) pm_store_gp(pm_sh, blockDim.x >> lg, F, args.gp_part);
+    if (WANT_P) store_param_part(pm_sh, blockDim.x >> lg, F, args.param_part);
 }
 
 // Rows that are not a whole number of aligned 16-byte vectors: one warp per work item, lane = feature.
 template <typename T, typename I, int MODE, int FORM, int PMODE, bool WANT_P>
 __global__ void __launch_bounds__(256, 1)
-power_mean_scalar_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, PmArgs args, int64_t n_rows,
+power_mean_scalar_kernel(const I* __restrict__ rowptr, const I* __restrict__ col, AggrArgs args, int64_t n_rows,
                          LongRowPlan plan) {
     using Fm = SmForms<FORM>;
     extern __shared__ float pm_sh[];
@@ -307,9 +260,8 @@ power_mean_scalar_kernel(const I* __restrict__ rowptr, const I* __restrict__ col
     const int64_t item = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
     int64_t row = 0, begin = 0, end = 0;
     bool is_chunk = false;
-    const bool active = decode_item(item, rowptr, n_rows, plan, row, begin, end, is_chunk);   // warp-uniform
+    const bool active = aggr_item<WANT_P>(item, rowptr, n_rows, plan, row, begin, end, is_chunk);   // warp-uniform
     if (!active && !WANT_P) return;
-    if (!active) row = begin = end = 0;                  // an idle group still writes its (zero) grad_p row
     const bool row_term = active && (!is_chunk || begin == static_cast<int64_t>(ldg_idx(rowptr + row)));
     const float deg = active ? pm_deg(rowptr, row) : 1.0f;
     const int64_t F = args.feat;
@@ -317,55 +269,55 @@ power_mean_scalar_kernel(const I* __restrict__ rowptr, const I* __restrict__ col
     const T* a = static_cast<const T*>(args.a);
     T* out = static_cast<T*>(args.out);
     for (int64_t f = lane; f < F; f += 32) {
-        const float pv = PMODE == kPmPNone ? 1.0f : __ldg(args.p + (PMODE == kPmPChannel ? f : 0));
+        const float pv = PMODE == kParamNone ? 1.0f : __ldg(args.param + (PMODE == kParamChannel ? f : 0));
         float acc = 0.0f, cc = 0.0f, gp = 0.0f, rx = 0.0f, rG = 0.0f;
-        if (MODE == kPmDst && active) {
+        if (MODE == kSweepDst && active) {
             float t = 0.0f;
             rG = pm_node<PMODE, WANT_P>(ElemTraits<T>::to_float(static_cast<const T*>(args.g)[row * F + f]),
                                         ElemTraits<T>::to_float(static_cast<const T*>(args.o)[row * F + f]),
-                                        args.M[row * F + f], deg, pv, args.lo, args.hi, t);
+                                        args.saved[row * F + f], deg, pv, args.lo, args.hi, t);
             if (row_term) gp = t;
         }
-        if (MODE == kPmSrc) rx = ElemTraits<T>::to_float(x[row * F + f]);
+        if (MODE == kSweepSrc) rx = ElemTraits<T>::to_float(x[row * F + f]);
 #pragma unroll 2
         for (int64_t e = begin; e < end; ++e) {
             const int64_t c = static_cast<int64_t>(ldg_idx(col + e));
-            const int64_t id = (Fm::kA || (MODE == kPmDst && out)) ? pm_eid<I>(args, e) : 0;
-            const float xv = MODE == kPmSrc ? rx : (Fm::kX ? ElemTraits<T>::to_float(x[c * F + f]) : 0.0f);
+            const int64_t id = (Fm::kA || (MODE == kSweepDst && out)) ? aggr_eid<I>(args, e) : 0;
+            const float xv = MODE == kSweepSrc ? rx : (Fm::kX ? ElemTraits<T>::to_float(x[c * F + f]) : 0.0f);
             const float av = Fm::kA ? ElemTraits<T>::to_float(a[id * F + f]) : 0.0f;
             bool on;
             const float m = sm_message<T, FORM>(xv, av, args.eps, on);
-            if (MODE == kPmFwd) {
+            if (MODE == kSweepFwd) {
                 pm_kahan(acc, cc, pm_term<T, PMODE>(m, pv, args.lo, args.hi));
             } else {
-                float gm = pm_grad<PMODE, WANT_P>(m, MODE == kPmSrc ? args.G[c * F + f] : rG, pv, args.lo, args.hi, gp);
+                float gm = pm_grad<PMODE, WANT_P>(m, MODE == kSweepSrc ? args.G[c * F + f] : rG, pv, args.lo, args.hi, gp);
                 if (Fm::kRelu && !on) gm = 0.0f;
-                if (MODE == kPmSrc) acc = __fadd_rn(acc, gm);
+                if (MODE == kSweepSrc) acc = __fadd_rn(acc, gm);
                 else if (out) out[id * F + f] = ElemTraits<T>::from_float(gm);
             }
         }
         if (WANT_P) pm_sh[(threadIdx.x >> 5) * F + f] = gp;
-        if (MODE == kPmDst || !active) continue;
-        if (MODE == kPmFwd) acc = __fsub_rn(acc, cc);
+        if (MODE == kSweepDst || !active) continue;
+        if (MODE == kSweepFwd) acc = __fsub_rn(acc, cc);
         if (is_chunk) {
             plan.partials[item * F + f] = acc;
             continue;
         }
-        if (MODE == kPmFwd) {
+        if (MODE == kSweepFwd) {
             float Mv;
             out[row * F + f] = ElemTraits<T>::from_float(pm_final<T, PMODE>(acc, deg, pv, args.lo, args.hi, Mv));
-            if (args.M) args.M[row * F + f] = Mv;
+            if (args.saved) args.saved[row * F + f] = Mv;
         } else {
             out[row * F + f] = ElemTraits<T>::from_float(acc);
         }
     }
-    if (WANT_P) pm_store_gp(pm_sh, blockDim.x >> 5, F, args.gp_part);
+    if (WANT_P) store_param_part(pm_sh, blockDim.x >> 5, F, args.param_part);
 }
 
 // Sum the partials of every long row in chunk order and write out and M.
 template <typename T, typename I, int PMODE>
 __global__ void __launch_bounds__(256)
-power_mean_combine_kernel(const I* __restrict__ rowptr, PmArgs args, LongRowPlan plan) {
+power_mean_combine_kernel(const I* __restrict__ rowptr, AggrArgs args, LongRowPlan plan) {
     const int64_t j = blockIdx.x;
     if (j >= plan.n_long) return;
     const int64_t F = args.feat;
@@ -374,12 +326,12 @@ power_mean_combine_kernel(const I* __restrict__ rowptr, PmArgs args, LongRowPlan
     const float deg = pm_deg(rowptr, row);
     T* out = static_cast<T*>(args.out);
     for (int64_t f = threadIdx.x; f < F; f += blockDim.x) {
-        const float pv = PMODE == kPmPNone ? 1.0f : __ldg(args.p + (PMODE == kPmPChannel ? f : 0));
+        const float pv = PMODE == kParamNone ? 1.0f : __ldg(args.param + (PMODE == kParamChannel ? f : 0));
         float S = 0.0f;
         for (int64_t c = c0; c < c1; ++c) S = __fadd_rn(S, plan.partials[c * F + f]);
         float Mv;
         out[row * F + f] = ElemTraits<T>::from_float(pm_final<T, PMODE>(S, deg, pv, args.lo, args.hi, Mv));
-        if (args.M) args.M[row * F + f] = Mv;
+        if (args.saved) args.saved[row * F + f] = Mv;
     }
 }
 
@@ -387,186 +339,72 @@ power_mean_combine_kernel(const I* __restrict__ rowptr, PmArgs args, LongRowPlan
 // one fp32 partial row per CTA.
 template <typename T, typename I, int PMODE, bool WANT_P>
 __global__ void __launch_bounds__(256)
-power_mean_node_kernel(const I* __restrict__ rowptr, PmArgs args, int64_t n_dst) {
+power_mean_node_kernel(const I* __restrict__ rowptr, AggrArgs args, int64_t n_dst) {
     const int64_t F = args.feat;
     const int64_t r0 = static_cast<int64_t>(blockIdx.x) * kPmNodeRows;
     const int64_t r1 = r0 + kPmNodeRows < n_dst ? r0 + kPmNodeRows : n_dst;
     const T* g = static_cast<const T*>(args.g);
     const T* o = static_cast<const T*>(args.o);
     for (int64_t f = threadIdx.x; f < F; f += blockDim.x) {
-        const float pv = PMODE == kPmPNone ? 1.0f : __ldg(args.p + (PMODE == kPmPChannel ? f : 0));
+        const float pv = PMODE == kParamNone ? 1.0f : __ldg(args.param + (PMODE == kParamChannel ? f : 0));
         float gp = 0.0f;
         for (int64_t r = r0; r < r1; ++r)
             args.G[r * F + f] = pm_node<PMODE, WANT_P>(ElemTraits<T>::to_float(g[r * F + f]),
                                                        ElemTraits<T>::to_float(o[r * F + f]),
-                                                       PMODE == kPmPNone ? 0.0f : args.M[r * F + f], pm_deg(rowptr, r),
+                                                       PMODE == kParamNone ? 0.0f : args.saved[r * F + f], pm_deg(rowptr, r),
                                                        pv, args.lo, args.hi, gp);
-        if (WANT_P) args.gp_part[static_cast<int64_t>(blockIdx.x) * F + f] = gp;
+        if (WANT_P) args.param_part[static_cast<int64_t>(blockIdx.x) * F + f] = gp;
     }
 }
 
-// ---------------------------------------------------------------- host-side dispatch
-template <typename T>
-bool pm_vec_ok(const PmArgs& a, const LongRowPlan& plan) {
-    return (a.feat * sizeof(T)) % 16 == 0 && aligned16(a.x) && aligned16(a.a) && aligned16(a.p) && aligned16(a.g) &&
-           aligned16(a.o) && aligned16(a.M) && aligned16(a.G) && aligned16(a.out) &&
-           (plan.n_chunks == 0 || aligned16(plan.partials));
-}
+struct PowerMeanOp {
+    static constexpr const char* kName = "power_mean";
+    static constexpr const char* kParam = "p";
+    static constexpr bool collects(int mode) { return mode != kSweepFwd; }
+    template <typename T, typename I, int MODE, int FORM, int PMODE, bool WANT_P>
+    static auto vec() { return power_mean_kernel<T, I, MODE, FORM, PMODE, WANT_P>; }
+    template <typename T, typename I, int MODE, int FORM, int PMODE, bool WANT_P>
+    static auto scalar() { return power_mean_scalar_kernel<T, I, MODE, FORM, PMODE, WANT_P>; }
+    template <typename T, typename I, int PMODE>
+    static void combine(const I* rowptr, const AggrArgs& args, const LongRowPlan& plan, cudaStream_t s) {
+        power_mean_combine_kernel<T, I, PMODE><<<static_cast<unsigned>(plan.n_long), 256, 0, s>>>(rowptr, args, plan);
+    }
+};
 
-// CTAs of the sweep that pm_launch runs, so that the caller can place the grad_p partials.
-template <typename T>
-int64_t pm_grid(const PmArgs& a, const LongRowPlan& plan, int64_t n_rows, int& lg, bool& vec) {
-    const int64_t items = plan.n_chunks + n_rows;
-    vec = pm_vec_ok<T>(a, plan);
-    if (vec) {
-        lane_group_shape<1>(static_cast<int>(a.feat * sizeof(T) / 16), [&](auto G, auto) {
-            lg = 0;
-            while ((1 << lg) < decltype(G)::value) ++lg;
-        });
-        return ceil_div(items, 128 >> lg);
-    }
-    lg = 5;
-    return ceil_div(items, 8);
-}
-
-template <typename T, typename I, int MODE, int FORM, int PMODE, bool WANT_P>
-int pm_launch(const I* rowptr, const I* col, const PmArgs& args, int64_t n_rows, const LongRowPlan& plan,
-              cudaStream_t stream) {
-    int lg;
-    bool vec;
-    const int64_t grid = pm_grid<T>(args, plan, n_rows, lg, vec);
-    if (grid == 0) return B200MP_OK;
-    const size_t smem = WANT_P ? static_cast<size_t>(vec ? (128 >> lg) : 8) * args.feat * sizeof(float) : 0;
-    if (smem > kPmMaxSmem) {
-        set_error("power_mean: grad_p of %lld channels needs %zu bytes of shared memory per CTA (at most %zu)",
-                  static_cast<long long>(args.feat), smem, kPmMaxSmem);
-        return B200MP_ERR_UNSUPPORTED;
-    }
-    if (vec) {
-        auto k = power_mean_kernel<T, I, MODE, FORM, PMODE, WANT_P>;
-        if (smem > 48 * 1024) B200MP_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                                    static_cast<int>(smem)));
-        k<<<static_cast<unsigned>(grid), 128, smem, stream>>>(rowptr, col, args, n_rows,
-                                                              static_cast<int>(args.feat * sizeof(T) / 16), lg, plan);
-    } else {
-        auto k = power_mean_scalar_kernel<T, I, MODE, FORM, PMODE, WANT_P>;
-        if (smem > 48 * 1024) B200MP_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                                    static_cast<int>(smem)));
-        k<<<static_cast<unsigned>(grid), 256, smem, stream>>>(rowptr, col, args, n_rows, plan);
-    }
-    B200MP_LAUNCH_CHECK();
-    if (MODE != kPmDst && plan.n_long > 0) {
-        if (MODE == kPmFwd)
-            power_mean_combine_kernel<T, I, PMODE><<<static_cast<unsigned>(plan.n_long), 256, 0, stream>>>(rowptr, args,
-                                                                                                          plan);
-        else
-            csr_combine_kernel<T, I, B200MP_SUM><<<static_cast<unsigned>(plan.n_long), 256, 0, stream>>>(
-                rowptr, static_cast<T*>(args.out), args.feat, false, false, plan, nullptr);
-        B200MP_LAUNCH_CHECK();
-    }
-    return B200MP_OK;
-}
-
-template <typename T, typename I, int MODE, int FORM>
-int pm_dispatch_p(const I* rowptr, const I* col, const PmArgs& args, int pmode, bool want_p, int64_t n_rows,
-                  const LongRowPlan& plan, cudaStream_t s) {
-    if constexpr (MODE != kPmFwd) {
-        if (want_p && pmode == kPmPScalar) return pm_launch<T, I, MODE, FORM, kPmPScalar, true>(rowptr, col, args, n_rows, plan, s);
-        if (want_p) return pm_launch<T, I, MODE, FORM, kPmPChannel, true>(rowptr, col, args, n_rows, plan, s);
-    }
-    if (pmode == kPmPScalar) return pm_launch<T, I, MODE, FORM, kPmPScalar, false>(rowptr, col, args, n_rows, plan, s);
-    if (pmode == kPmPChannel) return pm_launch<T, I, MODE, FORM, kPmPChannel, false>(rowptr, col, args, n_rows, plan, s);
-    return pm_launch<T, I, MODE, FORM, kPmPNone, false>(rowptr, col, args, n_rows, plan, s);
-}
-
-template <typename T, typename I, int MODE>
-int pm_typed(const void* rowptr_, const void* col_, PmArgs args, int form, int pmode, bool want_p, int64_t n_rows,
-             LongRowPlan plan, cudaStream_t s) {
-    const I* rowptr = static_cast<const I*>(rowptr_);
-    const I* col = static_cast<const I*>(col_);
-    switch (form) {
-        case kSmX: return pm_dispatch_p<T, I, MODE, kSmX>(rowptr, col, args, pmode, want_p, n_rows, plan, s);
-        case kSmXRelu: return pm_dispatch_p<T, I, MODE, kSmXRelu>(rowptr, col, args, pmode, want_p, n_rows, plan, s);
-        case kSmXARelu: return pm_dispatch_p<T, I, MODE, kSmXARelu>(rowptr, col, args, pmode, want_p, n_rows, plan, s);
-        default:
-            if (MODE == kPmSrc) break;                    // rows-only messages have no source operand
-            return pm_dispatch_p<T, I, MODE, kSmA>(rowptr, col, args, pmode, want_p, n_rows, plan, s);
-    }
-    set_error("power_mean: the transposed sweep needs x");
-    return B200MP_ERR_INVALID_ARG;
-}
-
-// Sweep CTAs of a grad_p-collecting sweep over n_rows rows (an upper bound over both kernels: a vector CTA holds at
-// least 4 work items, a scalar CTA 8), and the node kernel's CTAs.
-inline int64_t pm_sweep_ctas(int64_t n_rows, int64_t n_chunks) { return ceil_div(n_rows + n_chunks, 4); }
+// The node kernel's CTAs over n_node destination rows.
 inline int64_t pm_node_ctas(int64_t n_node) { return ceil_div(n_node, kPmNodeRows); }
 
-// Fold `parts` fp32 partial rows at ws into grad_p (zeros when there are none).
-inline int pm_fold(float* ws, int64_t parts, float* grad_p, int64_t feat, cudaStream_t s) {
-    if (parts == 0) return cudaMemsetAsync(grad_p, 0, feat * sizeof(float), s) == cudaSuccess ? B200MP_OK : B200MP_ERR_CUDA;
-    return b200mp_column_sum(ws, grad_p, ws + parts * feat, b200mp_column_sum_parts(parts), parts, feat, B200MP_F32, s);
-}
-
+// The node kernel, then the transposed sweep; grad_p from the node kernel's partial rows followed by the sweep's.
 template <typename T, typename I>
-int pm_dst(const void* rowptr, const void* col, PmArgs a, int form, int p_mode, float* grad_p, float* ws,
-           int64_t n_rows, LongRowPlan plan, cudaStream_t s) {
-    int lg;
-    bool vec;
-    const int64_t ctas = pm_grid<T>(a, plan, n_rows, lg, vec);
-    a.gp_part = ws;
-    const int rc = pm_typed<T, I, kPmDst>(rowptr, col, a, form, p_mode, grad_p != nullptr, n_rows, plan, s);
-    if (rc != B200MP_OK || grad_p == nullptr) return rc;
-    return pm_fold(ws, ctas, grad_p, a.feat, s);
-}
-
-template <typename T, typename I>
-int pm_src(const void* rowptr, const void* rowptr_t, const void* col_t, PmArgs a, int form, int p_mode, float* grad_p,
-           float* ws, int64_t n_src, int64_t n_dst, LongRowPlan plan, cudaStream_t s) {
+int pm_src(const void* rowptr, const void* rowptr_t, const void* col_t, AggrArgs a, int form, int p_mode, float* grad_p,
+           float* ws, int64_t n_src, int64_t n_dst, const LongRowPlan& plan, cudaStream_t s) {
     const int64_t F = a.feat;
     a.G = ws;
+    SweepShape sh;
+    if (int rc = sweep_shape<PowerMeanOp, T>(a, plan, n_src, grad_p != nullptr, sh)) return rc;
     float* parts = ws + n_dst * F;
     const int64_t node_ctas = pm_node_ctas(n_dst);
-    a.gp_part = parts;
+    a.param_part = parts;
     if (node_ctas > 0) {
-        if (grad_p == nullptr) {
-            if (p_mode == kPmPScalar)
-                power_mean_node_kernel<T, I, kPmPScalar, false><<<static_cast<unsigned>(node_ctas), 256, 0, s>>>(
-                    static_cast<const I*>(rowptr), a, n_dst);
-            else if (p_mode == kPmPChannel)
-                power_mean_node_kernel<T, I, kPmPChannel, false><<<static_cast<unsigned>(node_ctas), 256, 0, s>>>(
-                    static_cast<const I*>(rowptr), a, n_dst);
-            else
-                power_mean_node_kernel<T, I, kPmPNone, false><<<static_cast<unsigned>(node_ctas), 256, 0, s>>>(
-                    static_cast<const I*>(rowptr), a, n_dst);
-        } else if (p_mode == kPmPScalar) {
-            power_mean_node_kernel<T, I, kPmPScalar, true><<<static_cast<unsigned>(node_ctas), 256, 0, s>>>(
-                static_cast<const I*>(rowptr), a, n_dst);
-        } else {
-            power_mean_node_kernel<T, I, kPmPChannel, true><<<static_cast<unsigned>(node_ctas), 256, 0, s>>>(
-                static_cast<const I*>(rowptr), a, n_dst);
-        }
+        const unsigned grid = static_cast<unsigned>(node_ctas);
+        auto node = [&](auto k) { k<<<grid, 256, 0, s>>>(static_cast<const I*>(rowptr), a, n_dst); };
+        if (grad_p == nullptr && p_mode == kParamScalar) node(power_mean_node_kernel<T, I, kParamScalar, false>);
+        else if (grad_p == nullptr && p_mode == kParamChannel) node(power_mean_node_kernel<T, I, kParamChannel, false>);
+        else if (grad_p == nullptr) node(power_mean_node_kernel<T, I, kParamNone, false>);
+        else if (p_mode == kParamScalar) node(power_mean_node_kernel<T, I, kParamScalar, true>);
+        else node(power_mean_node_kernel<T, I, kParamChannel, true>);
         B200MP_LAUNCH_CHECK();
     }
-    int lg;
-    bool vec;
-    const int64_t ctas = n_src > 0 ? pm_grid<T>(a, plan, n_src, lg, vec) : 0;
-    a.gp_part = parts + node_ctas * F;
-    if (n_src > 0) {
-        const int rc = pm_typed<T, I, kPmSrc>(rowptr_t, col_t, a, form, p_mode, grad_p != nullptr, n_src, plan, s);
-        if (rc != B200MP_OK) return rc;
-    }
-    return grad_p == nullptr ? B200MP_OK : pm_fold(parts, node_ctas + ctas, grad_p, F, s);
+    a.param_part = parts + node_ctas * F;
+    if (int rc = aggr_typed<PowerMeanOp, T, I, kSweepSrc>(rowptr_t, col_t, a, form, p_mode, grad_p != nullptr, n_src,
+                                                          plan, sh, s))
+        return rc;
+    return grad_p == nullptr ? B200MP_OK : fold_param_parts(parts, node_ctas + sh.grid, grad_p, F, s);
 }
 
 }  // namespace b200mp
 
 using namespace b200mp;
-
-#define B200MP_CHECK_PM()                                                                                       \
-    B200MP_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && n_edges >= 0 && feat >= 0);                                  \
-    B200MP_CHECK_ARG(message == 0 || message == 1);                                                             \
-    B200MP_CHECK_ARG(p_mode >= 0 && p_mode <= 2 && (p_mode == 0 || (p && clamp_min > 0.0f && clamp_max >= clamp_min))); \
-    B200MP_CHECK_ARG(message == 1 ? x != nullptr : (x == nullptr) != (edge_rows == nullptr))
 
 extern "C" int b200mp_power_mean_csr(const void* rowptr, const void* col, const void* perm, const void* x,
                                      const void* edge_rows, const float* p, void* out, float* mean, int64_t n_rows,
@@ -574,21 +412,26 @@ extern "C" int b200mp_power_mean_csr(const void* rowptr, const void* col, const 
                                      float clamp_min, float clamp_max, const int64_t* long_rows,
                                      const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks, int64_t chunk,
                                      float* partials, int idx_dtype, int val_dtype, void* stream) {
-    B200MP_CHECK_PM();
+    if (int rc = check_aggr_args(n_rows, n_cols, n_edges, feat, message, x, edge_rows, p_mode, p, true, clamp_min,
+                                 clamp_max))
+        return rc;
     LongRowPlan plan;
     if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, partials, true)) return rc;
     if (n_rows == 0 || feat == 0) return B200MP_OK;
     B200MP_CHECK_ARG(rowptr && out);
     B200MP_CHECK_ARG(n_edges == 0 || x == nullptr || col);
-    const PmArgs a{x, edge_rows, p, perm, nullptr, nullptr, mean, nullptr, out, nullptr, feat, eps, clamp_min, clamp_max};
+    const AggrArgs a{x, edge_rows, p, perm, nullptr, nullptr, mean, nullptr, out, nullptr, feat, eps, clamp_min,
+                     clamp_max, false};
     return dispatch_val_idx(val_dtype, idx_dtype, "power_mean_csr", [&](auto tv, auto ti) {
-        return pm_typed<decltype(tv), decltype(ti), kPmFwd>(rowptr, col, a, sm_form(x, edge_rows, message), p_mode, false,
-                                                          n_rows, plan, static_cast<cudaStream_t>(stream));
+        return aggr_sweep<PowerMeanOp, decltype(tv), decltype(ti), kSweepFwd>(
+            rowptr, col, a, sm_form(x, edge_rows, message), p_mode, n_rows, plan, static_cast<cudaStream_t>(stream));
     });
 }
 
+// The grad_p partial rows are an upper bound over both sweep kernels (a vector CTA holds at least 4 work items, a
+// scalar CTA 8), after the node kernel's.
 extern "C" int64_t b200mp_power_mean_workspace(int64_t n_node, int64_t n_rows, int64_t n_chunks, int64_t feat) {
-    const int64_t parts = pm_node_ctas(n_node) + pm_sweep_ctas(n_rows, n_chunks);
+    const int64_t parts = pm_node_ctas(n_node) + ceil_div(n_rows + n_chunks, 4);
     return (n_node + parts + b200mp_column_sum_parts(parts)) * feat;
 }
 
@@ -600,7 +443,9 @@ extern "C" int b200mp_power_mean_backward_dst(const void* rowptr, const void* co
                                               float clamp_max, const int64_t* long_rows, const int64_t* chunk_ptr,
                                               int64_t n_long_rows, int64_t n_chunks, int64_t chunk, int idx_dtype,
                                               int val_dtype, void* stream) {
-    B200MP_CHECK_PM();
+    if (int rc = check_aggr_args(n_rows, n_cols, n_edges, feat, message, x, edge_rows, p_mode, p, true, clamp_min,
+                                 clamp_max))
+        return rc;
     B200MP_CHECK_ARG(grad_p == nullptr || (p_mode != 0 && workspace));
     LongRowPlan plan;
     if (int rc = make_plan(plan, long_rows, chunk_ptr, n_long_rows, n_chunks, chunk, nullptr, false)) return rc;
@@ -612,11 +457,12 @@ extern "C" int b200mp_power_mean_backward_dst(const void* rowptr, const void* co
     }
     B200MP_CHECK_ARG(rowptr && out && grad_out && (p_mode == 0 || mean));
     B200MP_CHECK_ARG(n_edges == 0 || x == nullptr || col);
-    const PmArgs a{x, edge_rows, p, perm, grad_out, out, const_cast<float*>(mean), nullptr, grad_edge_rows, nullptr,
-                   feat, eps, clamp_min, clamp_max};
+    const AggrArgs a{x, edge_rows, p, perm, grad_out, out, const_cast<float*>(mean), nullptr, grad_edge_rows, nullptr,
+                     feat, eps, clamp_min, clamp_max, false};
     return dispatch_val_idx(val_dtype, idx_dtype, "power_mean_backward_dst", [&](auto tv, auto ti) {
-        return pm_dst<decltype(tv), decltype(ti)>(rowptr, col, a, sm_form(x, edge_rows, message), p_mode, grad_p,
-                                                  workspace, n_rows, plan, static_cast<cudaStream_t>(stream));
+        return aggr_dst<PowerMeanOp, decltype(tv), decltype(ti)>(rowptr, col, a, sm_form(x, edge_rows, message), p_mode,
+                                                                 grad_p, workspace, n_rows, plan,
+                                                                 static_cast<cudaStream_t>(stream));
     });
 }
 
@@ -629,8 +475,9 @@ extern "C" int b200mp_power_mean_backward_src(const void* rowptr, const void* ro
                                               const int64_t* chunk_ptr, int64_t n_long_rows, int64_t n_chunks,
                                               int64_t chunk, float* partials, int idx_dtype, int val_dtype,
                                               void* stream) {
-    const int64_t n_rows = n_src, n_cols = n_dst;
-    B200MP_CHECK_PM();
+    if (int rc = check_aggr_args(n_src, n_dst, n_edges, feat, message, x, edge_rows, p_mode, p, true, clamp_min,
+                                 clamp_max))
+        return rc;
     B200MP_CHECK_ARG(x != nullptr);
     B200MP_CHECK_ARG(grad_p == nullptr || p_mode != 0);
     LongRowPlan plan;
@@ -640,8 +487,8 @@ extern "C" int b200mp_power_mean_backward_src(const void* rowptr, const void* ro
     B200MP_CHECK_ARG(workspace && rowptr && rowptr_t && (n_src == 0 || grad_x));
     B200MP_CHECK_ARG(n_dst == 0 || (out && grad_out && (p_mode == 0 || mean)));
     B200MP_CHECK_ARG(n_edges == 0 || (col_t && (edge_rows == nullptr || perm_t)));
-    const PmArgs a{x, edge_rows, p, perm_t, grad_out, out, const_cast<float*>(mean), nullptr, grad_x, nullptr, feat,
-                   eps, clamp_min, clamp_max};
+    const AggrArgs a{x, edge_rows, p, perm_t, grad_out, out, const_cast<float*>(mean), nullptr, grad_x, nullptr, feat,
+                     eps, clamp_min, clamp_max, false};
     return dispatch_val_idx(val_dtype, idx_dtype, "power_mean_backward_src", [&](auto tv, auto ti) {
         return pm_src<decltype(tv), decltype(ti)>(rowptr, rowptr_t, col_t, a, sm_form(x, edge_rows, message), p_mode,
                                                   grad_p, workspace, n_src, n_dst, plan,

@@ -296,6 +296,43 @@ def aggregate_cg_uv(graph: CSRGraph, uv: Tensor, c: Optional[Tensor] = None, red
                               "mean" if reduce == "mean" else "sum")
 
 
+def _param_aggr_operands(graph, x: Optional[Tensor], a: Optional[Tensor], w, name: str, what: str):
+    """The operands of softmax_aggregate and power_mean_aggregate: (x, a, w, where, want_saved).  `where` holds the
+    sweep's (rowptr, col, perm, plan, n_edges, graph); w (t or p) becomes None for a Python 1 (the reference then
+    skips the multiply, basic.py:207, or both clamps and pows, basic.py:285,290), ATen's fp32 scalar for another
+    number, or a contiguous fp32 tensor of 1 or F elements; want_saved: a backward will need the saved plane."""
+    if isinstance(graph, CSRGraph):
+        where = (graph.rowptr, graph.col, graph.perm, graph.plan, graph.num_edges, graph)
+        if x is not None and x.size(0) != graph.num_src:
+            raise ValueError(f"x has {x.size(0)} rows but the graph has {graph.num_src} source nodes")
+    else:
+        if x is not None:
+            raise ValueError("a (ptr, plan) message layout takes the messages as `a`, not x")
+        ptr, plan = graph
+        where = (ptr, None, None, plan, a.size(0), None)
+    ref = x if x is not None else a
+    if ref is None or ref.dim() != 2:
+        raise ValueError(f"{what} takes two-dimensional x or a")
+    if isinstance(w, Tensor):
+        ww = w.reshape(-1).float().contiguous()
+        if ww.numel() not in (1, ref.size(1)):
+            raise ValueError(f"{name} must have 1 or {ref.size(1)} elements, got {w.numel()}")
+    elif float(w) == 1.0:
+        ww = None
+    else:
+        ww = torch.full((1, ), float(w), dtype=torch.float32, device=ref.device)
+    x = None if x is None else x.contiguous()
+    a = None if a is None else a.contiguous()
+    want_saved = torch.is_grad_enabled() and any(v is not None and v.requires_grad for v in (x, a, ww))
+    return x, a, ww, where, want_saved
+
+
+def _sum_over_out_edges(graph: CSRGraph, grad_a: Tensor) -> Tensor:
+    """grad_x[j] = the sum of grad_a over j's out-edges, by the segment sum over the transposed CSR (perm_t is the
+    caller's edge id of each transposed slot)."""
+    return ops.spmm_csr(graph.rowptr_t, graph.perm_t, None, grad_a, graph.num_src, "sum", graph.plan_t)
+
+
 class _SoftmaxAggregate(torch.autograd.Function):
     """sum_e softmax_e(t * m_e) * m_e per destination and feature (csrc/softmax_aggr.cu).  The only saved state is
     the fp32 lse plane; the backward recomputes m, z and p.  The destination sweep gives grad_a and grad_t; grad_x is
@@ -326,8 +363,7 @@ class _SoftmaxAggregate(torch.autograd.Function):
         if need_x:
             graph.build_transpose()
             if ga is not None:
-                # grad_x[j] = the sum of grad_a over j's out-edges: perm_t is the caller's edge id of each transposed slot
-                gx = ops.spmm_csr(graph.rowptr_t, graph.perm_t, None, ga, graph.num_src, "sum", graph.plan_t)
+                gx = _sum_over_out_edges(graph, ga)
             else:
                 gx = ops.softmax_aggr_backward_src(graph.rowptr_t, graph.col_t, graph.perm_t, x, a, t, out, lse,
                                                    grad_out, ctx.message, ctx.eps, ctx.semi, graph.plan_t)
@@ -347,29 +383,7 @@ def softmax_aggregate(graph, x: Optional[Tensor], a: Optional[Tensor] = None, t=
     whose values the kernel reads on the device in fp32, so a learnable t adds no host sync; t * m is formed in fp32
     and rounded to the messages' dtype, and t's gradient has t's shape and dtype.  semi_grad: the softmax
     weights carry no gradient (t gets none).  Empty rows give 0."""
-    if isinstance(graph, CSRGraph):
-        where = (graph.rowptr, graph.col, graph.perm, graph.plan, graph.num_edges, graph)
-        if x is not None and x.size(0) != graph.num_src:
-            raise ValueError(f"x has {x.size(0)} rows but the graph has {graph.num_src} source nodes")
-    else:
-        if x is not None:
-            raise ValueError("a (ptr, plan) message layout takes the messages as `a`, not x")
-        ptr, plan = graph
-        where = (ptr, None, None, plan, a.size(0), None)
-    ref = x if x is not None else a
-    if ref is None or ref.dim() != 2:
-        raise ValueError("softmax_aggregate takes two-dimensional x or a")
-    if isinstance(t, Tensor):
-        tt = t.reshape(-1).float().contiguous()
-        if tt.numel() not in (1, ref.size(1)):
-            raise ValueError(f"t must have 1 or {ref.size(1)} elements, got {t.numel()}")
-    elif float(t) == 1.0:
-        tt = None                                                          # basic.py:207: no multiply
-    else:
-        tt = torch.full((1, ), float(t), dtype=torch.float32, device=ref.device)   # ATen's fp32 scalar
-    x = None if x is None else x.contiguous()
-    a = None if a is None else a.contiguous()
-    want_lse = torch.is_grad_enabled() and any(v is not None and v.requires_grad for v in (x, a, tt))
+    x, a, tt, where, want_lse = _param_aggr_operands(graph, x, a, t, "t", "softmax_aggregate")
     return _SoftmaxAggregate.apply(x, a, tt, where, float(eps), message, bool(semi_grad), want_lse)
 
 
@@ -400,8 +414,7 @@ class _PowerMeanAggregate(torch.autograd.Function):
         if need_x:
             graph.build_transpose()
             if ga is not None:
-                # grad_x[j] = the sum of grad_a over j's out-edges: perm_t is the caller's edge id of each transposed slot
-                gx = ops.spmm_csr(graph.rowptr_t, graph.perm_t, None, ga, graph.num_src, "sum", graph.plan_t)
+                gx = _sum_over_out_edges(graph, ga)
             else:
                 gx, gp = ops.power_mean_backward_src(rowptr, graph.rowptr_t, graph.col_t, graph.perm_t, x, a, p, out,
                                                      mean, grad_out, ctx.message, ctx.eps, ctx.lo, ctx.hi, need_p,
@@ -424,29 +437,7 @@ def power_mean_aggregate(graph, x: Optional[Tensor], a: Optional[Tensor] = None,
     reference does: a plain mean) or a tensor of 1 or F elements whose values the kernel reads on the device in fp32,
     so a learnable p adds no host sync; p's gradient has p's shape and dtype.  With p, clamp_min must be positive and
     clamp_max may be None (no upper bound).  An empty row gives clamp_min ^ (1 / p), or 0 without p."""
-    if isinstance(graph, CSRGraph):
-        where = (graph.rowptr, graph.col, graph.perm, graph.plan, graph.num_edges, graph)
-        if x is not None and x.size(0) != graph.num_src:
-            raise ValueError(f"x has {x.size(0)} rows but the graph has {graph.num_src} source nodes")
-    else:
-        if x is not None:
-            raise ValueError("a (ptr, plan) message layout takes the messages as `a`, not x")
-        ptr, plan = graph
-        where = (ptr, None, None, plan, a.size(0), None)
-    ref = x if x is not None else a
-    if ref is None or ref.dim() != 2:
-        raise ValueError("power_mean_aggregate takes two-dimensional x or a")
-    if isinstance(p, Tensor):
-        pp = p.reshape(-1).float().contiguous()
-        if pp.numel() not in (1, ref.size(1)):
-            raise ValueError(f"p must have 1 or {ref.size(1)} elements, got {p.numel()}")
-    elif float(p) == 1.0:
-        pp = None                                                          # basic.py:285,290: no clamp, no pow
-    else:
-        pp = torch.full((1, ), float(p), dtype=torch.float32, device=ref.device)   # ATen's fp32 scalar
-    x = None if x is None else x.contiguous()
-    a = None if a is None else a.contiguous()
-    want_mean = torch.is_grad_enabled() and any(v is not None and v.requires_grad for v in (x, a, pp))
+    x, a, pp, where, want_mean = _param_aggr_operands(graph, x, a, p, "p", "power_mean_aggregate")
     return _PowerMeanAggregate.apply(x, a, pp, where, float(eps), message, clamp_min, clamp_max, want_mean)
 
 

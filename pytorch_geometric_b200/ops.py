@@ -423,8 +423,7 @@ def edge_relu_backward_edge(rowptr: Tensor, perm: Optional[Tensor], grad_out: Te
     grad = torch.empty(n_edges, F, dtype=grad_out.dtype, device=grad_out.device)
     if n_edges == 0:
         return grad
-    pargs = (_p(plan.long_rows), _p(plan.chunk_ptr), plan.n_long, plan.n_chunks, plan.chunk) \
-        if plan is not None and plan.n_long else (None, None, 0, 0, 0)
+    pargs = _plan_rows(plan)
     _timed("edge_relu_backward_edge", 1, lib().b200mp_edge_relu_backward_edge, _p(rowptr), _p(perm), _p(grad_out),
            _p(mask), _p(grad), rowptr.numel() - 1, F, REDUCE[reduce], *pargs, it, _vdt(grad_out), _stream())
     return grad
@@ -579,9 +578,12 @@ def cg_backward_src(rowptr_t: Tensor, col_t: Tensor, perm_t: Tensor, val_t: Opti
 SOFTMAX_MESSAGES = {"identity": 0, "relu_eps": 1}
 
 
-def _softmax_aggr_args(x: Optional[Tensor], a: Optional[Tensor], t: Optional[Tensor], message: str, n_edges: int):
-    """Check the operands of the softmax-aggregation sweeps; returns (F, message code, t_mode).  x: [n_src, F] or
-    None; a: [n_edges, F] in the caller's edge order or None, contiguous, one dtype; t: None or fp32 [1] / [F]."""
+def _softmax_aggr_args(x: Optional[Tensor], a: Optional[Tensor], w: Optional[Tensor], message: str, n_edges: int,
+                       clamp: Optional[tuple] = None):
+    """Check the operands of the softmax- and power-mean-aggregation sweeps; returns (F, message code, mode of w), and
+    with power mean's clamp = (clamp_min, clamp_max) also (lo, hi).  x: [n_src, F] or None; a: [n_edges, F] in the
+    caller's edge order or None, contiguous, one dtype; w (t or p): None or fp32 [1] / [F]; with p, clamp_min > 0 and
+    clamp_max None (no upper bound) or >= clamp_min."""
     if message not in SOFTMAX_MESSAGES:
         raise ValueError(f"message must be one of {sorted(SOFTMAX_MESSAGES)}, got '{message}'")
     if message == "relu_eps" and x is None:
@@ -595,12 +597,18 @@ def _softmax_aggr_args(x: Optional[Tensor], a: Optional[Tensor], t: Optional[Ten
             raise ValueError(f"{name} must be a contiguous [N, {F}] tensor of dtype {ref.dtype}, got {tuple(v.shape)}")
     if a is not None and a.size(0) != n_edges:
         raise ValueError(f"edge rows must have {n_edges} rows, got {a.size(0)}")
-    t_mode = 0
-    if t is not None:
-        if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() not in (1, F):
-            raise ValueError(f"t must be a contiguous float32 tensor of 1 or {F} elements, got {tuple(t.shape)} {t.dtype}")
-        t_mode = 1 if t.numel() == 1 else 2
-    return F, SOFTMAX_MESSAGES[message], t_mode
+    mode = 0
+    if w is not None:
+        if w.dtype != torch.float32 or not w.is_contiguous() or w.numel() not in (1, F):
+            raise ValueError(f"t must be a contiguous float32 tensor of 1 or {F} elements, got {tuple(w.shape)} {w.dtype}")
+        mode = 1 if w.numel() == 1 else 2
+    if clamp is None:
+        return F, SOFTMAX_MESSAGES[message], mode
+    lo = 0.0 if clamp[0] is None else float(clamp[0])
+    hi = float("inf") if clamp[1] is None else float(clamp[1])
+    if w is not None and not (lo > 0.0 and hi >= lo):
+        raise ValueError(f"the power-mean sweep needs 0 < clamp_min <= clamp_max, got {clamp[0]} and {clamp[1]}")
+    return F, SOFTMAX_MESSAGES[message], mode, lo, hi
 
 
 def softmax_aggr_csr(rowptr: Tensor, col: Optional[Tensor], perm: Optional[Tensor], x: Optional[Tensor],
@@ -637,18 +645,15 @@ def softmax_aggr_backward_dst(rowptr: Tensor, col: Optional[Tensor], perm: Optio
     n_rows = rowptr.numel() - 1
     grad_a = torch.empty(n_edges, F, dtype=out.dtype, device=out.device) if want_grad_a else None
     grad_t = ws = None
-    n_chunks = plan.n_chunks if plan is not None and plan.n_long else 0
+    pargs = _plan_rows(plan)
     if want_grad_t:
         grad_t = torch.empty(F, dtype=torch.float32, device=out.device)
-        ws = torch.empty(max(int(lib().b200mp_softmax_aggr_workspace(n_rows, n_chunks, F)), 1), dtype=torch.float32,
+        ws = torch.empty(max(int(lib().b200mp_softmax_aggr_workspace(n_rows, pargs[3], F)), 1), dtype=torch.float32,
                          device=out.device)
-    # the destination sweep only splits long rows (nothing to combine): the plan without partials
-    pargs = _plan_args(None, F, out.device)[0] if not n_chunks else (_p(plan.long_rows), _p(plan.chunk_ptr), plan.n_long,
-                                                                     plan.n_chunks, plan.chunk)
     _timed("softmax_aggr_backward_dst", 3 if want_grad_t else 1, lib().b200mp_softmax_aggr_backward_dst, _p(rowptr),
            _p(col), _p(perm), _p(x), _p(a), _p(t), _p(out), _p(lse), _p(grad_out), _p(grad_a), _p(grad_t), _p(ws),
            n_rows, 0 if x is None else x.size(0), n_edges, F, msg, float(eps), t_mode, int(bool(semi_grad)),
-           *pargs[:5], it, _vdt(out), _stream())
+           *pargs, it, _vdt(out), _stream())
     return grad_a, grad_t
 
 
@@ -669,19 +674,6 @@ def softmax_aggr_backward_src(rowptr_t: Tensor, col_t: Tensor, perm_t: Tensor, x
     return grad_x
 
 
-def _power_mean_args(x: Optional[Tensor], a: Optional[Tensor], p: Optional[Tensor], message: str, n_edges: int,
-                     clamp_min: float, clamp_max: Optional[float]):
-    """Check the operands of the power-mean sweeps; returns (F, message code, p_mode, lo, hi).  As
-    _softmax_aggr_args, with p: None (a plain mean) or fp32 [1] / [F]; with p, clamp_min > 0 and clamp_max None
-    (no upper bound) or >= clamp_min."""
-    F, msg, p_mode = _softmax_aggr_args(x, a, p, message, n_edges)
-    hi = float("inf") if clamp_max is None else float(clamp_max)
-    lo = 0.0 if clamp_min is None else float(clamp_min)
-    if p is not None and not (lo > 0.0 and hi >= lo):
-        raise ValueError(f"the power-mean sweep needs 0 < clamp_min <= clamp_max, got {clamp_min} and {clamp_max}")
-    return F, msg, p_mode, lo, hi
-
-
 def power_mean_csr(rowptr: Tensor, col: Optional[Tensor], perm: Optional[Tensor], x: Optional[Tensor],
                    a: Optional[Tensor], p: Optional[Tensor], n_rows: int, n_edges: int, message: str = "identity",
                    eps: float = 0.0, clamp_min: float = 1e-4, clamp_max: Optional[float] = 100.0,
@@ -689,7 +681,7 @@ def power_mean_csr(rowptr: Tensor, col: Optional[Tensor], perm: Optional[Tensor]
     """out[i] = clamp(mean_e clamp(m_e)^p)^(1/p) over row i (b200mp_power_mean_csr), m_e as in softmax_aggr_csr; p None
     is a plain mean.  With want_mean also the fp32 plane of the means M the backward reads."""
     _cuda(rowptr, col, perm, x, a, p)
-    F, msg, p_mode, lo, hi = _power_mean_args(x, a, p, message, n_edges, clamp_min, clamp_max)
+    F, msg, p_mode, lo, hi = _softmax_aggr_args(x, a, p, message, n_edges, (clamp_min, clamp_max))
     it = _same_idx(rowptr, col, perm)
     ref = x if x is not None else a
     out = torch.empty(n_rows, F, dtype=ref.dtype, device=ref.device)
@@ -709,7 +701,7 @@ def power_mean_backward_dst(rowptr: Tensor, col: Optional[Tensor], perm: Optiona
     """Destination sweep of the power-mean backward: (grad_a [E, F] in the caller's edge order or None, grad_p [F]
     fp32 per-channel sums or None)."""
     _cuda(rowptr, col, perm, x, a, p, out, mean, grad_out)
-    F, msg, p_mode, lo, hi = _power_mean_args(x, a, p, message, n_edges, clamp_min, clamp_max)
+    F, msg, p_mode, lo, hi = _softmax_aggr_args(x, a, p, message, n_edges, (clamp_min, clamp_max))
     if want_grad_p and p is None:
         raise ValueError("grad_p needs p")
     it = _same_idx(rowptr, col, perm)
@@ -717,17 +709,14 @@ def power_mean_backward_dst(rowptr: Tensor, col: Optional[Tensor], perm: Optiona
     n_rows = rowptr.numel() - 1
     grad_a = torch.empty(n_edges, F, dtype=out.dtype, device=out.device) if want_grad_a else None
     grad_p = ws = None
-    n_chunks = plan.n_chunks if plan is not None and plan.n_long else 0
+    pargs = _plan_rows(plan)
     if want_grad_p:
         grad_p = torch.empty(F, dtype=torch.float32, device=out.device)
-        ws = torch.empty(max(int(lib().b200mp_power_mean_workspace(0, n_rows, n_chunks, F)), 1), dtype=torch.float32,
+        ws = torch.empty(max(int(lib().b200mp_power_mean_workspace(0, n_rows, pargs[3], F)), 1), dtype=torch.float32,
                          device=out.device)
-    # the destination sweep only splits long rows (nothing to combine): the plan without partials
-    pargs = _plan_args(None, F, out.device)[0] if not n_chunks else (_p(plan.long_rows), _p(plan.chunk_ptr), plan.n_long,
-                                                                     plan.n_chunks, plan.chunk)
     _timed("power_mean_backward_dst", 3 if want_grad_p else 1, lib().b200mp_power_mean_backward_dst, _p(rowptr),
            _p(col), _p(perm), _p(x), _p(a), _p(p), _p(out), _p(mean), _p(grad_out), _p(grad_a), _p(grad_p), _p(ws),
-           n_rows, 0 if x is None else x.size(0), n_edges, F, msg, float(eps), p_mode, lo, hi, *pargs[:5], it,
+           n_rows, 0 if x is None else x.size(0), n_edges, F, msg, float(eps), p_mode, lo, hi, *pargs, it,
            _vdt(out), _stream())
     return grad_a, grad_p
 
@@ -740,7 +729,7 @@ def power_mean_backward_src(rowptr: Tensor, rowptr_t: Tensor, col_t: Tensor, per
     per-channel sums or None).  rowptr: the destination CSR's, for the degrees."""
     _cuda(rowptr, rowptr_t, col_t, perm_t, x, a, p, out, mean, grad_out)
     E = col_t.numel()
-    F, msg, p_mode, lo, hi = _power_mean_args(x, a, p, message, E, clamp_min, clamp_max)
+    F, msg, p_mode, lo, hi = _softmax_aggr_args(x, a, p, message, E, (clamp_min, clamp_max))
     if want_grad_p and p is None:
         raise ValueError("grad_p needs p")
     it = _same_idx(rowptr, rowptr_t, col_t, perm_t)
@@ -868,12 +857,20 @@ def softmax_csr_backward(out: Tensor, grad_out: Tensor, ptr: Tensor, plan: Optio
     return g.view(out.shape)
 
 
+def _plan_rows(plan) -> tuple:
+    """(long_rows, chunk_ptr, n_long, n_chunks, chunk) for the C ABI: the plan of a sweep that splits long rows but has
+    nothing to combine, so takes no partials."""
+    if plan is None or not plan.n_long:
+        return (None, None, 0, 0, 0)
+    return (_p(plan.long_rows), _p(plan.chunk_ptr), plan.n_long, plan.n_chunks, plan.chunk)
+
+
 def _plan_args(plan, feat: int, device):
     """(long_rows, chunk_ptr, n_long, n_chunks, chunk, partials[n_chunks*feat]) for the C ABI."""
     if plan is None or not plan.n_long:
         return (None, None, 0, 0, 0, None), None
     part = plan.partials(feat, device)
-    return (_p(plan.long_rows), _p(plan.chunk_ptr), plan.n_long, plan.n_chunks, plan.chunk, _p(part)), part
+    return (*_plan_rows(plan), _p(part)), part
 
 
 def gat_fused_csr(rowptr: Tensor, col: Tensor, xh: Tensor, a_src: Tensor, a_dst: Tensor, heads: int, chan: int,

@@ -1,15 +1,9 @@
 """CPU tests of the power-mean aggregation and the fused GENConv: PowerMeanAggregation's constructor errors, parameters
 and repr against the reference, aggregation_resolver('powermean'), B200GENConv in plugin.conv.LAYERS and falling
-through to the reference bit for bit on CPU tensors and with hooks, the fusability predicates case by case, and the
-plan checks of the three power-mean entry points."""
-import re
-
-import numpy as np
+through to the reference bit for bit on CPU tensors and with hooks, and the fusability predicates case by case."""
 import pytest
 import torch
 
-import pytorch_geometric_b200 as pgb
-from pytorch_geometric_b200 import _build
 from pytorch_geometric_b200.nn import PowerMeanAggregation, aggregation_resolver
 from pytorch_geometric_b200.nn.aggr import power_mean_fusable
 
@@ -142,60 +136,3 @@ def test_mirror_constructor_errors_and_layout(tg, golden):
         ref = tg.nn.GENConv(ch, 16, **kw)
         assert [n for n, _ in conv.named_parameters()] == [n for n, _ in ref.named_parameters()], tag
     assert GENConv(8, 8, aggr="power").aggr == "powermean"
-
-
-# ---------------------------------------------------------------- plan checks of the C entry points
-pytestmark_plan = pytest.mark.skipif(torch.cuda.is_available(), reason="passes host buffers as device pointers")
-INVALID_ARG = -1
-PM_PLANS = ("power_mean_csr", "power_mean_backward_dst", "power_mean_backward_src")
-WRITES_PARTIALS = {"power_mean_csr": True, "power_mean_backward_dst": False, "power_mean_backward_src": True}
-SCALARS = {"n_rows": 4, "n_cols": 4, "n_src": 4, "n_dst": 4, "n_edges": 8, "feat": 8, "message": 1, "eps": 1e-7,
-           "p_mode": 1, "clamp_min": 1e-4, "clamp_max": 100.0, "plan_chunk": 4, "plan_n_long_rows": 0,
-           "plan_n_chunks": 0, "idx_dtype": 1, "val_dtype": 0}
-MALFORMED = {
-    "negative_long_rows": {"plan_n_long_rows": -1},
-    "negative_chunks": {"plan_n_long_rows": 1, "plan_n_chunks": -1},
-    "zero_chunk": {"plan_n_long_rows": 1, "plan_n_chunks": 1, "plan_chunk": 0},
-    "no_partials": {"plan_n_long_rows": 1, "plan_n_chunks": 1, "plan_partials": None},
-}
-_RAW = np.zeros(1 << 16, dtype=np.uint8)
-BUF = _RAW.ctypes.data + (-_RAW.ctypes.data) % 16
-with open(f"{_build.INCLUDE}/b200mp.h") as _f:
-    _HEADER = re.sub(r"/\*.*?\*/", "", _f.read(), flags=re.S)
-PROTOS = {m.group(1): [(re.findall(r"\w+", p)[-1], "*" in p) for p in m.group(2).split(",")]
-          for m in re.finditer(r"\bb200mp_(\w+)\s*\(([^)]*)\)\s*;", _HEADER)}
-
-
-def _call(name, **override):
-    args = []
-    for pname, is_ptr in PROTOS[name]:
-        if pname in override:
-            args.append(override[pname])
-        elif is_ptr:
-            args.append(None if pname == "stream" else BUF)
-        else:
-            args.append(SCALARS[pname])
-    return getattr(pgb.lib(), "b200mp_" + name)(*args)
-
-
-@pytestmark_plan
-@pytest.mark.parametrize("long_rows", [False, True])
-@pytest.mark.parametrize("name", PM_PLANS)
-def test_power_mean_valid_plan_passes_the_checks(name, long_rows):
-    override = {"plan_n_long_rows": 1, "plan_n_chunks": 1} if long_rows else {}
-    assert _call(name, **override) != INVALID_ARG, pgb.lib().b200mp_last_error()
-
-
-@pytestmark_plan
-@pytest.mark.parametrize("case", sorted(MALFORMED))
-@pytest.mark.parametrize("name", PM_PLANS)
-def test_power_mean_malformed_plan_is_rejected(name, case):
-    if case == "no_partials" and not WRITES_PARTIALS[name]:
-        pytest.skip("this sweep writes no partials")
-    assert _call(name, **MALFORMED[case]) == INVALID_ARG, pgb.lib().b200mp_last_error()
-
-
-@pytestmark_plan
-@pytest.mark.parametrize("name", PM_PLANS)
-def test_power_mean_rejects_a_non_positive_clamp_min(name):
-    assert _call(name, clamp_min=0.0) == INVALID_ARG

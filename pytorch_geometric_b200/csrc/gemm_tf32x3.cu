@@ -14,7 +14,7 @@
 // and one TF32 MMA of equal issue cost instead of three TF32 ones -- fp32-class accuracy at half the TF32 tensor rate.
 // (The "tf32x3" names of the entry points date from the three-product form.)
 //
-// Structure (one persistent CTA per SM, 384 threads = three warpgroups, 128 x BN output tiles, BK = 32):
+// Structure (one persistent CTA per SM, 384 threads = three warpgroups, 256 x BN output tiles, BK = 32):
 //   warpgroup 0, warp 0   TMA producer: one thread streams the raw fp32 A and B tiles into a ring of shared-memory
 //                         stages (cp.async.bulk.tensor.2d, mbarrier complete_tx)
 //   warpgroup 0, warps 1-3  B preparation, only when B is MN-major or arrives unsplit: split (and transpose) the
@@ -24,13 +24,14 @@
 //                         (W_hi, W_lo of the forward) is packed once per call into a global correction matrix
 //                         (pack_corr_kernel); TMA then writes hi and correction tiles in the wgmma layout, and the
 //                         descriptors point at the stage itself.
-//   warpgroups 1-2        consumers, 64 output rows each.  Per k-block they issue 4 k-steps x (one
-//                         wgmma.m64nBNk16.f32.bf16.bf16 correction, then one wgmma.m64nBNk8.f32.tf32.tf32 hi*hi)
-//                         (A from registers, B from shared memory) and, while those run, load and split the A
-//                         fragments of the next k-block -- possibly the next tile's --
-//                         into the other of two register sets; then wgmma.wait_group 0, and one thread per
-//                         warpgroup releases the stage (and split slot).  (Keeping a group in flight across
-//                         k-blocks with wait_group 1 made ptxas serialize every wgmma: C7518.)
+//   warpgroups 1-2        consumers, 128 output rows each, as two m64 halves that share the stage's B tile.  Per
+//                         k-block each issues 4 k-steps x 2 halves x (one wgmma.m64nBNk16.f32.bf16.bf16 correction,
+//                         then one wgmma.m64nBNk8.f32.tf32.tf32 hi*hi) as one group (A from registers, B from shared
+//                         memory), then wgmma.wait_group 0, releases the stage (and split slot), stores the tile if it
+//                         was its last k-block, and loads and splits the next k-block's A fragments.  The two run
+//                         independently on the same stages, so one's group keeps the tensor cores busy while the other
+//                         drains, loads or stores.  (Keeping a group in flight across k-blocks with wait_group 1 made
+//                         ptxas serialize every wgmma: C7518.)
 //                         The epilogue adds the bias, applies ReLU and stores the fragments with masked rows.
 // Operands may be K-major (row-major [rows, K]) or MN-major (row-major [K, rows]), so all three products
 // read x, g and W exactly as they lie in HBM (no transposes in global memory).
@@ -42,7 +43,7 @@
 
 namespace b200mp {
 
-constexpr int kBM = 128;             // output rows per CTA tile (two m64 warpgroups)
+constexpr int kBM = 256;             // output rows per CTA tile (two warpgroups x two m64 halves)
 constexpr int kBK = 32;              // fp32 elements of K per stage = one 128-byte swizzle row
 constexpr int kMaxStages = 4;
 constexpr int kSplitSlots = 2;       // ring of split B buffers written by the B-preparation warps
@@ -100,6 +101,46 @@ __device__ __forceinline__ void fence_regs(float (&d)[R]) {
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+// Stall trace, compiled in only with -DB200MP_GEMM_TRACE (benchmarks/gemm_stalls.py builds such a library on the side):
+// clock64 totals per role, summed over CTAs into g_gemm_trace by one thread per consumer warpgroup / producer thread /
+// preparation warp.  The normal build keeps an empty GemmTrace and untimed calls.
+enum TraceSlot {
+    kTrFullWait,      // consumers: waiting on bar_full (A, and B when read from the stage) or bar_sfull (prepared B)
+    kTrMmaWait,       // consumers: wgmma.wait_group
+    kTrEpilogue,      // consumers: store_tile
+    kTrConsumer,      // consumers: whole loop
+    kTrEmptyWait,     // TMA producer: waiting on bar_empty
+    kTrProducer,      // TMA producer: whole loop
+    kTrPrepFullWait,  // B preparation: waiting on bar_full
+    kTrPrepSlotWait,  // B preparation: waiting on bar_sempty
+    kTrPrep,          // B preparation: whole loop
+    kTrSlots
+};
+#ifdef B200MP_GEMM_TRACE
+__device__ unsigned long long g_gemm_trace[kTrSlots];
+struct GemmTrace {
+    long long t[kTrSlots] = {};
+    __device__ void flush(bool leader) const {
+        if (leader)
+            for (int i = 0; i < kTrSlots; ++i) atomicAdd(&g_gemm_trace[i], static_cast<unsigned long long>(t[i]));
+    }
+};
+template <int SLOT, class F>
+__device__ __forceinline__ void traced(GemmTrace& tr, F&& f) {
+    const long long t0 = clock64();
+    f();
+    tr.t[SLOT] += clock64() - t0;
+}
+#else
+struct GemmTrace {
+    __device__ void flush(bool) const {}
+};
+template <int SLOT, class F>
+__device__ __forceinline__ void traced(GemmTrace&, F&& f) {
+    f();
+}
+#endif
+
 // A fragments of one k-block, split: [k-step][register].  Register i of the m64k8 tf32 fragment holds (row r or r+8,
 // k = t or t+4); register i of the m64k16 bf16 fragment holds the same row at bf16 positions 2k, 2k+1 -- so corr[j][i]
 // = pack(bf16(a_lo), bf16(a_hi)) of the thread's own element i, no shuffles.  Fenced like the accumulators, so that
@@ -244,7 +285,7 @@ __device__ __forceinline__ bool decode_tile(int w, const GemmArgs& args, const i
 template <int BN, bool B_MN, bool B_PRE>
 struct GemmPlan {
     static constexpr bool kDirectB = B_PRE && !B_MN;               // wgmma reads B straight from the stage
-    static constexpr uint32_t kABytes = kBM * kBK * 4;             // 16 KB
+    static constexpr uint32_t kABytes = kBM * kBK * 4;             // 32 KB
     static constexpr uint32_t kBBytes = BN * kBK * 4;
     static constexpr uint32_t kStageBytes = kABytes + (B_PRE ? 2 : 1) * kBBytes;
     static constexpr uint32_t kSplitBytes = kDirectB ? 0 : kSplitSlots * 2 * kBBytes;
@@ -258,7 +299,7 @@ struct GemmPlan {
 // A_MN / B_MN: operand is MN-major (stored row-major as [K, MN]); B_PRE: B arrives pre-split (tmap_b_hi, and tmap_b_lo
 // = the packed correction when K-major, lo when MN-major), else tmap_b_hi is the raw matrix and the B-preparation warps
 // split it.  An MN-major A arrives as
-// four [32 k][32 m] boxes with the 128B swizzle, so the column-wise fragment loads do not collide in one bank.
+// up to eight [32 k][32 m] boxes (one per 32 rows of the tile) with the 128B swizzle, so the column-wise fragment loads do not collide in one bank.
 template <int BN, bool A_MN, bool B_MN, bool B_PRE, bool GROUPED>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
@@ -280,7 +321,7 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     auto bar_sempty = [&](int s) { return bars + 8u * (2 * kStages + kSplitSlots + s); };
 
     __shared__ int tile_prefix[GROUPED ? kMaxSegments + 2 : 1];
-    if (GROUPED && threadIdx.x == 32) {                          // tiles of 128 rows per segment, exclusive prefix
+    if (GROUPED && threadIdx.x == 32) {                          // tiles of kBM rows per segment, exclusive prefix
         int acc = 0;
         for (int r = 0; r < args.n_seg; ++r) {
             tile_prefix[r] = acc;
@@ -310,14 +351,16 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     };
 
     // registers: the producer and B-preparation warpgroup gives up what the two MMA warpgroups need beyond the even
-    // share of 168 (accumulators + two A fragment sets); 128 x 56 + 256 x 224 <= 64 K
+    // share of 168 (two m64 accumulators + one A fragment set per half); 128 x 40 + 256 x 232 <= 64 K
     if (wg == 0) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 56;" ::: "memory");
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
         const int warp = threadIdx.x >> 5;
+        GemmTrace tr;
         if (threadIdx.x == 0) {
             // ===================== TMA producer =====================
             int stage = 0;
             uint32_t phase = 0;
+            traced<kTrProducer>(tr, [&] {
             for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
                 Tile t;
                 decode_tile<GROUPED>(w, args, tile_prefix, t);
@@ -326,17 +369,19 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
                 int kb0, kb1;
                 k_range(t, kb0, kb1);
                 for (int kb = kb0; kb < kb1; ++kb) {
-                    bar_wait(bar_empty(stage), phase ^ 1u);
+                    traced<kTrEmptyWait>(tr, [&] { bar_wait(bar_empty(stage), phase ^ 1u); });
                     const uint32_t sa = smem_base + stage * kStageBytes;
                     const uint32_t sb = sa + kABytes;
-                    bar_expect_tx(bar_full(stage), kStageBytes);
                     if (A_MN) {
-#pragma unroll
-                        for (int b = 0; b < kBM / 32; ++b) tma_load_2d(sa + b * 4096u, &tmap_a, m0 + 32 * b, kb * kBK, bar_full(stage));
-                    } else if (kb < args.k_blocks_a1) {
-                        tma_load_2d(sa, &tmap_a, kb * kBK, m0, bar_full(stage));
+                        // only the 32-row boxes that hold rows of the tile (a 128-row output fills half of one); the
+                        // rows of the stage past them are never stored
+                        const int boxes = (t.rows + 31) / 32;
+                        bar_expect_tx(bar_full(stage), kStageBytes - (kBM / 32 - boxes) * 4096u);
+                        for (int b = 0; b < boxes; ++b) tma_load_2d(sa + b * 4096u, &tmap_a, m0 + 32 * b, kb * kBK, bar_full(stage));
                     } else {
-                        tma_load_2d(sa, &tmap_a2, (kb - args.k_blocks_a1) * kBK, m0, bar_full(stage));
+                        bar_expect_tx(bar_full(stage), kStageBytes);
+                        if (kb < args.k_blocks_a1) tma_load_2d(sa, &tmap_a, kb * kBK, m0, bar_full(stage));
+                        else tma_load_2d(sa, &tmap_a2, (kb - args.k_blocks_a1) * kBK, m0, bar_full(stage));
                     }
                     if (B_MN) {
                         tma_load_2d(sb, &tmap_b_hi, n0, b_row0 + kb * kBK, bar_full(stage));
@@ -348,6 +393,8 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
                     if (++stage == kStages) { stage = 0; phase ^= 1u; }
                 }
             }
+            });
+            tr.flush(true);
         } else if (!kDirectB && warp >= 1) {
             // ============ B preparation: stage -> prepared slot (hi, corr), K-major 128B swizzle ============
             // corr word of element (n, k) = pack(bf16(b_hi), bf16(b_lo)) at the byte offset of the fp32 element: a
@@ -355,14 +402,15 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
             const int pt = threadIdx.x - 32;                    // 0 .. 95
             int stage = 0, slot = 0;
             uint32_t phase = 0, sphase = 0;
+            traced<kTrPrep>(tr, [&] {
             for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
                 Tile t;
                 decode_tile<GROUPED>(w, args, tile_prefix, t);
                 int kb0, kb1;
                 k_range(t, kb0, kb1);
                 for (int kb = kb0; kb < kb1; ++kb) {
-                    bar_wait(bar_full(stage), phase);
-                    bar_wait(bar_sempty(slot), sphase ^ 1u);
+                    traced<kTrPrepFullWait>(tr, [&] { bar_wait(bar_full(stage), phase); });
+                    traced<kTrPrepSlotWait>(tr, [&] { bar_wait(bar_sempty(slot), sphase ^ 1u); });
                     const unsigned char* sb = smem_gen + stage * kStageBytes + kABytes;
                     unsigned char* bh = smem_gen + (split_base - smem_base) + slot * 2 * kBBytes;
                     unsigned char* bc = bh + kBBytes;
@@ -411,33 +459,38 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
                     if (++slot == kSplitSlots) { slot = 0; sphase ^= 1u; }
                 }
             }
+            });
+            tr.flush(lane == 0);
         }
         return;
     }
 
     // ===================== consumers: warpgroups 1 and 2 =====================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;" ::: "memory");
-    const int row_base = (wg - 1) * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // fragment rows row_base, +8
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    // this warpgroup's 128 rows of the tile are two m64 halves; fragment rows of half hf: row_base + 64 hf, +8
+    const int row_base = (wg - 1) * 128 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
     const int kq = lane & 3;
     const bool signal = (threadIdx.x & 127) == 0;               // releases stages / slots for its warpgroup
     int w = blockIdx.x;
     if (w >= n_work) return;
 
-    // (A) fragments of this warpgroup's 64 rows from a raw stage, split in registers
-    auto load_a = [&](AFrag& f, int stage) {
+    // (A) fragments of this warpgroup's two 64-row halves from a raw stage, split in registers
+    auto load_a = [&](AFrag (&f)[2], int stage) {
         const unsigned char* sa = smem_gen + stage * kStageBytes;
 #pragma unroll
-        for (int j = 0; j < kBK / 8; ++j) {
+        for (int hf = 0; hf < 2; ++hf)
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int r = row_base + (i & 1) * 8, k = j * 8 + kq + (i >> 1) * 4;
-                const float v = A_MN ? *reinterpret_cast<const float*>(sa + (r >> 5) * 4096 + sw128_offset(k, r & 31))
-                                     : *reinterpret_cast<const float*>(sa + sw128_offset(r, k));
-                const float h = rn_tf32(v);
-                f.hi[j][i] = __float_as_uint(h);
-                f.corr[j][i] = pack_bf16x2(v - h, h);
+            for (int j = 0; j < kBK / 8; ++j) {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int r = row_base + hf * 64 + (i & 1) * 8, k = j * 8 + kq + (i >> 1) * 4;
+                    const float v = A_MN ? *reinterpret_cast<const float*>(sa + (r >> 5) * 4096 + sw128_offset(k, r & 31))
+                                         : *reinterpret_cast<const float*>(sa + sw128_offset(r, k));
+                    const float h = rn_tf32(v);
+                    f[hf].hi[j][i] = __float_as_uint(h);
+                    f[hf].corr[j][i] = pack_bf16x2(v - h, h);
+                }
             }
-        }
     };
 
     Tile t;
@@ -447,10 +500,14 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     int kb = kb0;
     int stage = 0, slot = 0;                                    // ring positions of k-block kb
     uint32_t phase = 0, sphase = 0;
-    float acc[kAcc];
-    AFrag f0, f1;
-    bar_wait(bar_full(stage), phase);
-    load_a(f0, stage);
+    float acc[2][kAcc];
+    AFrag f[2];
+    GemmTrace tr;
+#ifdef B200MP_GEMM_TRACE
+    const long long tr_start = clock64();
+#endif
+    traced<kTrFullWait>(tr, [&] { bar_wait(bar_full(stage), phase); });
+    load_a(f, stage);
 
     auto release = [&](int st, int sl) {
         if (signal) {
@@ -465,78 +522,91 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         float* out = second ? args.c2 : args.c;
         const int64_t ldc = second ? args.ldc2 : args.ldc;
         const int col0 = (second ? nt - args.n_tiles_c1 : nt) * BN;
-        const int bias0 = nt * BN;
-        float* base = out + static_cast<int64_t>(tt.split) * args.m * ldc;
+        const float* bias = args.bias ? args.bias + nt * BN : nullptr;
+        float* base = out + static_cast<int64_t>(tt.split) * args.m * ldc + tt.m0 * ldc + col0;   // the tile's (0, 0)
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int r = row_base + h * 8;
-            const bool keep = r < tt.rows;
-            float* dst = base + (tt.m0 + r) * ldc + col0;
+        for (int hf = 0; hf < 2; ++hf)
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                const int c = j * 8 + 2 * kq;
-                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-                if (args.bias) {
-                    v0 += __ldg(args.bias + bias0 + c);
-                    v1 += __ldg(args.bias + bias0 + c + 1);
+            for (int h = 0; h < 2; ++h) {
+                const int r = row_base + hf * 64 + h * 8;
+                const bool keep = r < tt.rows;
+                float* dst = base + r * ldc;
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int c = j * 8 + 2 * kq;
+                    float v0 = acc[hf][4 * j + 2 * h], v1 = acc[hf][4 * j + 2 * h + 1];
+                    if (bias) {
+                        v0 += __ldg(bias + c);
+                        v1 += __ldg(bias + c + 1);
+                    }
+                    if (args.relu) {
+                        v0 = fmaxf(v0, 0.0f);
+                        v1 = fmaxf(v1, 0.0f);
+                    }
+                    if (keep) *reinterpret_cast<float2*>(dst + c) = make_float2(v0, v1);
                 }
-                if (args.relu) {
-                    v0 = fmaxf(v0, 0.0f);
-                    v1 = fmaxf(v1, 0.0f);
-                }
-                if (keep) *reinterpret_cast<float2*>(dst + c) = make_float2(v0, v1);
             }
-        }
     };
-    // One k-block: cur holds its A fragments; on return nxt holds those of the next k-block (false: no more work).
-    auto step = [&](AFrag& cur, AFrag& nxt) -> bool {
+    // One k-block: f holds its A fragments; on return f holds those of the next k-block (false: no more work).
+    auto step = [&]() -> bool {
         uint32_t b_hi;
         if (kDirectB) {
             b_hi = smem_base + stage * kStageBytes + kABytes;
         } else {
-            bar_wait(bar_sfull(slot), sphase);
+            traced<kTrFullWait>(tr, [&] { bar_wait(bar_sfull(slot), sphase); });
             b_hi = split_base + slot * 2 * kBBytes;
         }
         const uint32_t b_corr = b_hi + kBBytes;
-        // 4 k-steps x (bf16 correction pair, tf32 hi*hi), small terms first; the k16 bf16 step and the k8 tf32 step
-        // both advance 32 B along the swizzle row
-        fence_frag(cur);
+        // 4 k-steps x (bf16 correction pair, tf32 hi*hi) on each half, small terms first; the k16 bf16 step and the k8
+        // tf32 step both advance 32 B along the swizzle row.  Per accumulator the order is that of one m64 tile.
+        fence_frag(f[0]);
+        fence_frag(f[1]);
         wgmma_fence();
 #pragma unroll
         for (int j = 0; j < kBK / 8; ++j) {
-            wgmma_bf16<BN>(acc, cur.corr[j], smem_desc_sw128(b_corr + j * 32u), (kb > kb0 || j > 0) ? 1u : 0u);
-            wgmma_tf32<BN>(acc, cur.hi[j], smem_desc_sw128(b_hi + j * 32u), 1u);
+            const uint32_t scale = (kb > kb0 || j > 0) ? 1u : 0u;
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf) {
+                wgmma_bf16<BN>(acc[hf], f[hf].corr[j], smem_desc_sw128(b_corr + j * 32u), scale);
+                wgmma_tf32<BN>(acc[hf], f[hf].hi[j], smem_desc_sw128(b_hi + j * 32u), 1u);
+            }
         }
         wgmma_commit();
         const int cur_stage = stage, cur_slot = slot;
         if (++stage == kStages) { stage = 0; phase ^= 1u; }
         if (!kDirectB && ++slot == kSplitSlots) { slot = 0; sphase ^= 1u; }
         const bool tile_done = ++kb == kb1;
-        Tile tn = t;
         bool more = true;
         if (tile_done) {
             w += gridDim.x;
             more = w < n_work;
-            if (more) decode_tile<GROUPED>(w, args, tile_prefix, tn);
         }
-        if (more) {                                             // next A fragments, possibly the next tile's
-            fence_frag(nxt);
-            bar_wait(bar_full(stage), phase);
-            load_a(nxt, stage);
-        }
-        wgmma_wait_all();
-        fence_regs(acc);
+        traced<kTrMmaWait>(tr, [&] { wgmma_wait_all(); });
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
         release(cur_stage, cur_slot);
         if (tile_done) {
-            store_tile(t);
-            t = tn;
-            k_range(t, kb0, kb1);
-            kb = kb0;
+            traced<kTrEpilogue>(tr, [&] { store_tile(t); });
+            if (more) {
+                decode_tile<GROUPED>(w, args, tile_prefix, t);
+                k_range(t, kb0, kb1);
+                kb = kb0;
+            }
+        }
+        if (more) {                                             // next A fragments, possibly the next tile's
+            fence_frag(f[0]);
+            fence_frag(f[1]);
+            traced<kTrFullWait>(tr, [&] { bar_wait(bar_full(stage), phase); });
+            load_a(f, stage);
         }
         return more;
     };
-    while (step(f0, f1) && step(f1, f0)) {
+    while (step()) {
     }
+#ifdef B200MP_GEMM_TRACE
+    tr.t[kTrConsumer] += clock64() - tr_start;
+#endif
+    tr.flush(signal);
 }
 
 // w -> (rn_tf32(w), w - rn_tf32(w)) for the (small) weight matrix
@@ -739,7 +809,7 @@ static int run_pair(const float* a1, int64_t k1, const float* a2, int64_t k2, co
 static int run_grad_weight(const float* g, const float* x, float* gw, int64_t m, int64_t n, int64_t k, void* workspace,
                            int64_t workspace_bytes, cudaStream_t s) {
     const int bn = tile_n(k);
-    const int tiles = static_cast<int>((n / kBM) * (k / bn));
+    const int tiles = static_cast<int>(ceil_div(n, kBM) * (k / bn));
     const int64_t kblocks = ceil_div(m, kBK);
     if (kblocks > 0x7fffffffLL) return B200MP_ERR_UNSUPPORTED;
     int splits = num_sms() / tiles;
@@ -759,7 +829,7 @@ static int run_grad_weight(const float* g, const float* x, float* gw, int64_t m,
     args.c = static_cast<float*>(workspace);
     args.m = n;
     args.ldc = k;
-    args.n_tiles_m = static_cast<int>(n / kBM);
+    args.n_tiles_m = static_cast<int>(ceil_div(n, kBM));
     args.n_tiles_n = args.n_tiles_c1 = static_cast<int>(k / bn);
     args.k_blocks = static_cast<int>(kblocks);
     args.k_blocks_per_split = kbps;
@@ -775,6 +845,21 @@ static int run_grad_weight(const float* g, const float* x, float* gw, int64_t m,
 }  // namespace b200mp
 
 using namespace b200mp;
+
+#ifdef B200MP_GEMM_TRACE
+// trace build only (not part of the C ABI): copy the kTrSlots clock64 totals to out, then zero them if reset
+extern "C" int b200mp_gemm_trace_read(unsigned long long* out, int n, int reset) {
+    B200MP_CHECK_ARG(out && n == kTrSlots);
+    B200MP_CUDA(cudaDeviceSynchronize());
+    B200MP_CUDA(cudaMemcpyFromSymbol(out, g_gemm_trace, sizeof(unsigned long long) * kTrSlots));
+    if (reset) {
+        void* p = nullptr;
+        B200MP_CUDA(cudaGetSymbolAddress(&p, g_gemm_trace));
+        B200MP_CUDA(cudaMemset(p, 0, sizeof(unsigned long long) * kTrSlots));
+    }
+    return B200MP_OK;
+}
+#endif
 
 extern "C" int b200mp_split_tf32(const float* w, float* w_hi, float* w_lo, int64_t n, void* stream) {
     B200MP_CHECK_ARG(n >= 0);
@@ -858,7 +943,7 @@ extern "C" int b200mp_gemm_pair_tf32x3(const float* a1, int64_t k1, const float*
 }
 
 // out[ptr[r] : ptr[r+1]] = a[ptr[r] : ptr[r+1]] . B_r for every segment r in ONE persistent launch: work items are
-// (segment, 128-row tile inside the segment, 128-column tile); the tile -> segment map is rebuilt in shared memory from
+// (segment, 256-row tile inside the segment, 128-column tile); the tile -> segment map is rebuilt in shared memory from
 // the device-resident ptr, so the segment sizes never travel to the host.
 extern "C" int b200mp_segment_matmul_tf32x3(const float* a, const int64_t* ptr, int64_t n_seg, const float* b_hi, const float* b_lo,
                                             int b_layout, float* c, int64_t m, int64_t k, int64_t n, void* stream) {

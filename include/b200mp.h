@@ -417,6 +417,52 @@ int b200mp_power_mean_backward_src(const void* rowptr, const void* rowptr_t, con
                                    int64_t n_chunks, int64_t chunk, float* partials, int idx_dtype, int val_dtype,
                                    void* stream);
 
+/* ------------------------------------------------------------------ quantile aggregation (one selection sweep)
+ * Replaces: QuantileAggregation.forward / MedianAggregation (nn/aggr/quantile.py:71-130: a column-wise sort of the
+ * [E, F] messages, a stable sort of an expanded int64 [E, F] index and two gathers).  Per destination i (count_i
+ * in-edges from offset ptr_i = rowptr[i]), channel f and q = q[k] (fp32 on the device, n_q >= 1):
+ *   h = fl32(q fl32(count_i - 1)),  P = fl32(h + fl32(ptr_i))   (quantile.py:88; exact integer offsets once
+ *   ptr_i + count_i - 1 >= 2^24, where the reference's fp32 P leaves the group; every rank is then clamped into
+ *   [0, count_i - 1], as fl32(count_i - 1) may round up past 2^24)
+ *   interpolation 0 linear: l + (r - l) frac   1 lower: floor(P)   2 higher: ceil(P)   3 nearest: rint(P) (half to even)
+ *   4 midpoint: 0.5 l + 0.5 r   -- l, r the values of rank floor(P) - ptr_i and ceil(P) - ptr_i, frac = P - floor(P)
+ * Ranks order the messages by value (-0.0 == +0.0, NaN above +inf), ties by CSR slot (the caller's order).  Each op
+ * rounds as ATen's; bf16 linear writes fp32 (the reference's promotion), every other case the messages' dtype.  An
+ * empty row gives fill_value.  out: [n_rows, n_q * feat], row i = [q_0 | q_1 | ...] (quantile.py:125-129).
+ * Messages: x [n_cols, feat] gathered through col, or edge_rows [n_edges, feat] in the CALLER's order read through perm
+ * (NULL: the slot).  bits: NULL, or the saved state of the backward, b200mp_quantile_bits_words(...) uint32 words
+ * [n_edges (caller order), R n_q, ceil(feat / 32)], R = 2 for linear and midpoint (floor picks, then ceil picks) and 1
+ * otherwise; zeroed and written here.  plan_*: the destination CSR's long-row plan (b200mp_csr_plan_*): its rows are
+ * selected by one CTA per 32 channels; no partials.  csrc/quantile.cu states the algorithm. */
+int64_t b200mp_quantile_bits_words(int64_t n_edges, int64_t n_q, int interpolation, int64_t feat);
+int b200mp_quantile_csr(const void* rowptr, const void* col, const void* perm, const void* x, const void* edge_rows,
+                        const float* q, int64_t n_q, int interpolation, float fill_value, void* out, uint32_t* bits,
+                        int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t feat, const int64_t* plan_rows,
+                        const int64_t* plan_chunk_ptr, int64_t plan_n_long, int64_t plan_n_chunks, int64_t plan_chunk,
+                        int idx_dtype, int val_dtype, void* stream);
+/* The gradient of the edge rows, written densely in the caller's order (quantile.py's autograd: the sort, gathers and
+ * index_select backward): g = grad_out[i, k feat + f] (fp32 for bf16 linear, else the messages' dtype) goes to each
+ * picked element as g (lower, higher, nearest), round(0.5 g) (midpoint), or g - g frac and g frac (linear; bf16:
+ * round(round(g) - round(g frac)) and round(g frac)); an element's picks are summed over q in order, each add rounded,
+ * the floor picks' sum then plus the ceil picks'.  Reads only bits, q and grad_out.  plan_*: the destination CSR's plan
+ * (long rows split into chunks; no partials). */
+int b200mp_quantile_backward_dst(const void* rowptr, const void* perm, const float* q, int64_t n_q, int interpolation,
+                                 const uint32_t* bits, const void* grad_out, void* grad_edge_rows, int64_t n_rows,
+                                 int64_t n_edges, int64_t feat, const int64_t* plan_rows,
+                                 const int64_t* plan_chunk_ptr, int64_t plan_n_long, int64_t plan_n_chunks,
+                                 int64_t plan_chunk, int idx_dtype, int val_dtype, void* stream);
+/* grad_x of the gathered form by ONE sweep over the TRANSPOSED CSR: grad_x[j] = the fp32 sum, in transposed slot
+ * order, of the per-message gradient above over j's out-edges t (message perm_t[t], destination col_t[t]), read only
+ * where a bit is set; rounded once to the messages' dtype.  A long source row is summed per plan chunk and the chunk
+ * sums are folded in chunk order.  rowptr: the destination CSR's (offsets and counts).
+ * plan_*: the transposed CSR's plan, partials [plan_n_chunks, feat] fp32, folded in chunk order. */
+int b200mp_quantile_backward_src(const void* rowptr, const void* rowptr_t, const void* col_t, const void* perm_t,
+                                 const float* q, int64_t n_q, int interpolation, const uint32_t* bits,
+                                 const void* grad_out, void* grad_x, int64_t n_src, int64_t n_dst, int64_t n_edges,
+                                 int64_t feat, const int64_t* plan_rows, const int64_t* plan_chunk_ptr,
+                                 int64_t plan_n_long, int64_t plan_n_chunks, int64_t plan_chunk, float* plan_partials,
+                                 int idx_dtype, int val_dtype, void* stream);
+
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)
  * out[index[e], :] (+)= src[e, :] for an UNSORTED index.  Replaces utils/_scatter.py:14-138
  * (aten::scatter_add_ / scatter_reduce_, torch_scatter.scatter).  fp32 only.  `count` is a

@@ -66,6 +66,13 @@ _SIGS = {
                                                                          _INT, _INT, _P]),
     "b200mp_power_mean_backward_src": (_INT, [_P] * 13 + [_I64] * 4 + [_INT, _F, _INT, _F, _F, _P, _P, _I64, _I64, _I64,
                                                                          _P, _INT, _INT, _P]),
+    "b200mp_quantile_bits_words": (_I64, [_I64, _I64, _INT, _I64]),
+    "b200mp_quantile_csr": (_INT, [_P] * 6 + [_I64, _INT, _F, _P, _P] + [_I64] * 4 + [_P, _P, _I64, _I64, _I64, _INT,
+                                                                                  _INT, _P]),
+    "b200mp_quantile_backward_dst": (_INT, [_P] * 3 + [_I64, _INT, _P, _P, _P] + [_I64] * 3 + [_P, _P, _I64, _I64, _I64,
+                                                                                              _INT, _INT, _P]),
+    "b200mp_quantile_backward_src": (_INT, [_P] * 5 + [_I64, _INT, _P, _P, _P] + [_I64] * 4 + [_P, _P, _I64, _I64, _I64,
+                                                                                              _P, _INT, _INT, _P]),
     "b200mp_scatter_coo": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
     "b200mp_split_tf32": (_INT, [_P, _P, _P, _I64, _P]),
     "b200mp_split_tf32_transposed": (_INT, [_P, _P, _P, _I64, _I64, _P]),

@@ -441,6 +441,72 @@ def power_mean_aggregate(graph, x: Optional[Tensor], a: Optional[Tensor] = None,
     return _PowerMeanAggregate.apply(x, a, pp, where, float(eps), message, clamp_min, clamp_max, want_mean)
 
 
+class _QuantileAggregate(torch.autograd.Function):
+    """The q-quantiles of each destination's messages per channel (csrc/quantile.cu).  The only saved state is the
+    pick bits, one per (message, rank, channel).  grad_a comes from the destination sweep, grad_x of gathered messages
+    from one transposed sweep; each runs only when its output is needed."""
+
+    @staticmethod
+    def forward(ctx, x, a, q, where, interpolation: str, fill_value: float, want_bits: bool):
+        rowptr, col, perm, plan, n_edges, _ = where
+        out, bits = ops.quantile_csr(rowptr, col, perm, x, a, q, interpolation, fill_value, rowptr.numel() - 1,
+                                     n_edges, plan, want_bits)
+        ctx.where, ctx.interpolation = where, interpolation
+        ctx.dtype, ctx.feat = (x if x is not None else a).dtype, (x if x is not None else a).size(1)
+        ctx.save_for_backward(x, q, bits)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out: Tensor):
+        x, q, bits = ctx.saved_tensors
+        rowptr, col, perm, plan, n_edges, graph = ctx.where
+        need_x, need_a = ctx.needs_input_grad[:2]
+        gx = ga = None
+        if need_a:
+            ga = ops.quantile_backward_dst(rowptr, perm, q, ctx.interpolation, bits, grad_out, n_edges, ctx.feat,
+                                           ctx.dtype, plan)
+        if need_x:
+            graph.build_transpose()
+            gx = ops.quantile_backward_src(rowptr, graph.rowptr_t, graph.col_t, graph.perm_t, q, ctx.interpolation,
+                                           bits, grad_out, x, graph.plan_t)
+        return gx, ga, None, None, None, None, None
+
+
+def quantile_aggregate(graph, x: Optional[Tensor], a: Optional[Tensor], q, interpolation: str = "linear",
+                       fill_value: float = 0.0) -> Tensor:
+    """QuantileAggregation / MedianAggregation (nn/aggr/quantile.py:71-130) as one selection sweep: no sort, and
+    nothing float stored per message.
+
+        out[i, k F + f] = the q[k]-quantile of {m_e[f] : e = (j -> i)},   m_e = x[j] | a[e]
+
+    graph: a CSRGraph (x: [num_src, F] gathered per edge, or a: [E, F] in the caller's edge order), or (ptr, plan) for a
+    destination-sorted [E, F] message matrix `a` (x None).  q: a float32 tensor of Q values in [0, 1] on the messages'
+    device (the kernel reads it there, so a loaded state_dict takes effect with no host read), or a Python number or
+    list.  interpolation: linear, lower, higher, nearest or midpoint.  Ranks, order, ties and roundings are
+    csrc/quantile.cu's contract; bf16 'linear' returns float32.  Empty rows give fill_value.  Returns [N, Q * F]."""
+    if (x is None) == (a is None):
+        raise ValueError("quantile_aggregate takes exactly one of x and a")
+    if isinstance(graph, CSRGraph):
+        where = (graph.rowptr, graph.col if x is not None else None, graph.perm, graph.plan, graph.num_edges, graph)
+        if x is not None and x.size(0) != graph.num_src:
+            raise ValueError(f"x has {x.size(0)} rows but the graph has {graph.num_src} source nodes")
+    else:
+        if x is not None:
+            raise ValueError("a (ptr, plan) message layout takes the messages as `a`, not x")
+        ptr, plan = graph
+        where = (ptr, None, None, plan, a.size(0), None)
+    ref = x if x is not None else a
+    if ref.dim() != 2:
+        raise ValueError("quantile_aggregate takes two-dimensional x or a")
+    if not isinstance(q, Tensor):
+        q = torch.tensor(q if isinstance(q, (list, tuple)) else [q], dtype=torch.float32, device=ref.device)
+    qq = q.reshape(-1).contiguous()
+    x = None if x is None else x.contiguous()
+    a = None if a is None else a.contiguous()
+    want_bits = torch.is_grad_enabled() and ref.requires_grad
+    return _QuantileAggregate.apply(x, a, qq, where, interpolation, float(fill_value), want_bits)
+
+
 class _PNAAggregate(torch.autograd.Function):
     """PNAConv's aggregation of m_e = u_i + w_e, w_e = v_j (+ c_e) (csrc/pna.cu).  The sweep collects the statistics
     of w (b200mp_multi_aggr_csr on v, or b200mp_pna_edge_stats with c); the epilogue shifts them by u, applies the

@@ -1,6 +1,6 @@
 """Aggregation modules: mirrors of torch_geometric.nn.aggr.{Sum,Mean,Max,Min,Var,Std,Softmax,PowerMean}Aggregation
-(nn/aggr/base.py:102-185, basic.py:12-50,83-139,142-297), FusedAggregation (fused.py:20-336) and
-MultiAggregation (multi.py:14-200) on the sm_90a kernels.
+(nn/aggr/base.py:102-185, basic.py:12-50,83-139,142-297), {Quantile,Median}Aggregation (quantile.py:10-161),
+FusedAggregation (fused.py:20-336) and MultiAggregation (multi.py:14-200) on the sm_90a kernels.
 
 `__call__(x, index=None, ptr=None, dim_size=None, dim=-2)` has the reference's meaning and error
 behaviour.  Unlike the reference (base.py:177-180 only uses `ptr` in deterministic mode), the CSR
@@ -246,6 +246,77 @@ def _group_forward(fn, x, index, ptr, dim_size, index_sorted, **kw):
     return fn(CSRGraph(e, index, index.numel(), dim_size), None, x, **kw)
 
 
+class QuantileAggregation(Aggregation):
+    """The feature-wise q-quantile(s) of each group (nn/aggr/quantile.py:10-134), as one selection sweep over the
+    messages (functional.quantile_aggregate) instead of two sorts of the [E, F] matrix.  q is the reference's float32
+    buffer of shape [Q, 1], read on the device.  Ranks past 2^24 messages are exact, ties go to the earlier message and
+    an empty first group gives fill_value (the reference raises IndexError there): csrc/quantile.cu states the
+    contract.  Takes CUDA float32 / bfloat16 messages; other dtypes raise TypeError."""
+    interpolations = {"linear", "lower", "higher", "nearest", "midpoint"}
+
+    def __init__(self, q, interpolation: str = "linear", fill_value: float = 0.0):
+        super().__init__()
+        qs = [q] if not isinstance(q, (list, tuple)) else q
+        if len(qs) == 0:
+            raise ValueError("Provide at least one quantile value for `q`.")
+        if not all(0. <= quantile <= 1. for quantile in qs):
+            raise ValueError("`q` must be in the range [0, 1].")
+        if interpolation not in self.interpolations:
+            raise ValueError(f"Invalid interpolation method got ('{interpolation}')")
+        self._q = q
+        self.register_buffer("q", torch.tensor(qs).view(-1, 1))
+        self.interpolation = interpolation
+        self.fill_value = fill_value
+
+    def forward(self, x, index=None, ptr=None, dim_size=None, dim=-2, index_sorted=False):
+        d = dim + x.dim() if dim < 0 else dim
+        if index is None:
+            raise NotImplementedError("Aggregation requires 'index' to be specified")
+        if x.dtype not in (torch.float32, torch.bfloat16):
+            raise TypeError(f"QuantileAggregation takes float32 or bfloat16 messages, got {x.dtype}")
+        if self.q.dtype != torch.float32:
+            raise TypeError(f"QuantileAggregation needs a float32 q buffer, got {self.q.dtype}")
+        if dim_size is None:
+            dim_size = ptr.numel() - 1 if ptr is not None else (
+                ops.index_stats(index)[1] + 1 if index.numel() > 0 else 0)
+        xm = x.movedim(d, 0)
+        x2 = xm.reshape(xm.size(0), -1)
+        if x2.size(0) == 0:
+            out = torch.full((dim_size, self.q.numel() * x2.size(1)), self.fill_value, device=x.device,
+                             dtype=ops.quantile_out_dtype(x.dtype, self.interpolation))
+        else:
+            out = _group_forward(Fn.quantile_aggregate, x2, index, ptr, dim_size, index_sorted, q=self.q,
+                                 interpolation=self.interpolation, fill_value=self.fill_value)
+        return quantile_layout(out, self.q.numel(), x.shape, d)
+
+    def __repr__(self) -> str:
+        return f"{self.__class__.__name__}(q={self._q})"
+
+
+class MedianAggregation(QuantileAggregation):
+    """The feature-wise lower median of each group (nn/aggr/quantile.py:137-161): QuantileAggregation(0.5, 'lower')."""
+
+    def __init__(self, fill_value: float = 0.0):
+        super().__init__(0.5, "lower", fill_value)
+
+    def __repr__(self) -> str:
+        return f"{self.__class__.__name__}()"
+
+
+def quantile_layout(out: Tensor, n_q: int, shape, d: int) -> Tensor:
+    """The reference's layout (quantile.py:125-129) of a [N, Q * W] sweep result over x of `shape` aggregated along d
+    (W: every other dimension, in order): [..., N, Q * shape[d + 1], ...], [..., N, Q] when d is the last dimension,
+    and x's own shape with N at d for one q."""
+    rest = list(shape[:d]) + list(shape[d + 1:])
+    n = out.size(0)
+    out = out.view(n, n_q, *rest).movedim((0, 1), (d, d + 1))
+    if n_q == 1:
+        return out.reshape(*shape[:d], n, *shape[d + 1:])
+    if d + 1 < len(shape):
+        return out.reshape(*shape[:d], n, n_q * shape[d + 1], *shape[d + 2:])
+    return out.reshape(*shape[:d], n, n_q)
+
+
 class VarAggregation(Aggregation):
     """var = mean(x^2) - mean(x)^2 per group (nn/aggr/basic.py:83-111), one fused sweep."""
     fused_name = "var"
@@ -385,7 +456,7 @@ class MultiAggregation(Aggregation):
 def aggregation_resolver(name: str, **kwargs) -> Aggregation:
     table = {"sum": SumAggregation, "add": SumAggregation, "mean": MeanAggregation, "max": MaxAggregation,
              "min": MinAggregation, "var": VarAggregation, "std": StdAggregation, "softmax": SoftmaxAggregation,
-             "powermean": PowerMeanAggregation}
+             "powermean": PowerMeanAggregation, "median": MedianAggregation, "quantile": QuantileAggregation}
     if name not in table:
         raise ValueError(f"Could not resolve '{name}' among the aggregations on the hot path {sorted(table)}")
     return table[name](**kwargs)

@@ -747,6 +747,85 @@ def power_mean_backward_src(rowptr: Tensor, rowptr_t: Tensor, col_t: Tensor, per
     return grad_x, grad_p
 
 
+QUANTILE_INTERPOLATIONS = {"linear": 0, "lower": 1, "higher": 2, "nearest": 3, "midpoint": 4}
+
+
+def _quantile_args(ref: Tensor, q: Tensor, interpolation: str) -> Tuple[int, int, int]:
+    """(F, interpolation code, Q) of a quantile call: q a contiguous fp32 device tensor of Q >= 1 values."""
+    if interpolation not in QUANTILE_INTERPOLATIONS:
+        raise ValueError(f"interpolation must be one of {sorted(QUANTILE_INTERPOLATIONS)}, got '{interpolation}'")
+    if q.dtype != torch.float32 or not q.is_contiguous() or q.numel() < 1:
+        raise ValueError(f"q must be a contiguous float32 tensor of at least one value, got {tuple(q.shape)} {q.dtype}")
+    _vdt(ref)
+    if ref.dim() != 2 or not ref.is_contiguous():
+        raise ValueError(f"the messages must be a contiguous two-dimensional tensor, got {tuple(ref.shape)}")
+    return ref.size(1), QUANTILE_INTERPOLATIONS[interpolation], q.numel()
+
+
+def quantile_out_dtype(dtype: torch.dtype, interpolation: str) -> torch.dtype:
+    """The reference's result dtype: bf16 'linear' promotes to float32 through the fp32 frac."""
+    return torch.float32 if dtype == torch.bfloat16 and interpolation == "linear" else dtype
+
+
+def quantile_bits(n_edges: int, n_q: int, interpolation: str, feat: int, device) -> Tensor:
+    """The pick bits of one forward: [n_edges, R * n_q, ceil(feat / 32)] int32 words (b200mp_quantile_bits_words)."""
+    words = int(lib().b200mp_quantile_bits_words(n_edges, n_q, QUANTILE_INTERPOLATIONS[interpolation], feat))
+    return torch.empty(max(words, 1), dtype=torch.int32, device=device)
+
+
+def quantile_csr(rowptr: Tensor, col: Optional[Tensor], perm: Optional[Tensor], x: Optional[Tensor],
+                 a: Optional[Tensor], q: Tensor, interpolation: str, fill_value: float, n_rows: int, n_edges: int,
+                 plan: Optional[LongRowPlan] = None, want_bits: bool = False) -> Tuple[Tensor, Optional[Tensor]]:
+    """out[i, k F + f] = the q[k]-quantile of row i's messages in channel f (b200mp_quantile_csr): x[col[e]] or
+    a[perm[e]] (perm None: a[e]).  With want_bits also the pick bits the backward reads."""
+    _cuda(rowptr, col, perm, x, a, q)
+    if (x is None) == (a is None):
+        raise ValueError("the quantile sweep takes exactly one of x and the edge rows")
+    ref = x if x is not None else a
+    F, interp, Q = _quantile_args(ref, q, interpolation)
+    if a is not None and a.size(0) != n_edges:
+        raise ValueError(f"edge rows must have {n_edges} rows, got {a.size(0)}")
+    it = _same_idx(rowptr, col, perm)
+    out = torch.empty(n_rows, Q * F, dtype=quantile_out_dtype(ref.dtype, interpolation), device=ref.device)
+    bits = quantile_bits(n_edges, Q, interpolation, F, ref.device) if want_bits else None
+    pargs = _plan_rows(plan)
+    _timed("quantile_csr", (2 if pargs[2] else 1) + int(want_bits), lib().b200mp_quantile_csr, _p(rowptr), _p(col),
+           _p(perm), _p(x), _p(a), _p(q), Q, interp, float(fill_value), _p(out), _p(bits), n_rows,
+           0 if x is None else x.size(0), n_edges, F, *pargs, it, _vdt(ref), _stream())
+    return out, bits
+
+
+def quantile_backward_dst(rowptr: Tensor, perm: Optional[Tensor], q: Tensor, interpolation: str, bits: Tensor,
+                          grad_out: Tensor, n_edges: int, feat: int, dtype: torch.dtype,
+                          plan: Optional[LongRowPlan] = None) -> Tensor:
+    """The gradient of the edge rows [n_edges, feat] of `dtype`, in the caller's order (b200mp_quantile_backward_dst)."""
+    _cuda(rowptr, perm, q, bits, grad_out)
+    grad_a = torch.empty(n_edges, feat, dtype=dtype, device=grad_out.device)
+    _, interp, Q = _quantile_args(grad_a, q, interpolation)
+    grad_out = grad_out.to(quantile_out_dtype(dtype, interpolation)).contiguous()
+    it = _same_idx(rowptr, perm)
+    _timed("quantile_backward_dst", 1, lib().b200mp_quantile_backward_dst, _p(rowptr), _p(perm), _p(q), Q, interp,
+           _p(bits), _p(grad_out), _p(grad_a), rowptr.numel() - 1, n_edges, feat, *_plan_rows(plan), it,
+           _vdt(grad_a), _stream())
+    return grad_a
+
+
+def quantile_backward_src(rowptr: Tensor, rowptr_t: Tensor, col_t: Tensor, perm_t: Tensor, q: Tensor,
+                          interpolation: str, bits: Tensor, grad_out: Tensor, x: Tensor,
+                          plan_t: Optional[LongRowPlan] = None) -> Tensor:
+    """grad_x [n_src, F] of the gathered form by one transposed sweep (b200mp_quantile_backward_src)."""
+    _cuda(rowptr, rowptr_t, col_t, perm_t, q, bits, grad_out, x)
+    F, interp, Q = _quantile_args(x, q, interpolation)
+    grad_out = grad_out.to(quantile_out_dtype(x.dtype, interpolation)).contiguous()
+    it = _same_idx(rowptr, rowptr_t, col_t, perm_t)
+    grad_x = torch.empty_like(x)
+    pargs, _ = _plan_args(plan_t, F, x.device)
+    _timed("quantile_backward_src", 2 if pargs[2] else 1, lib().b200mp_quantile_backward_src, _p(rowptr),
+           _p(rowptr_t), _p(col_t), _p(perm_t), _p(q), Q, interp, _p(bits), _p(grad_out), _p(grad_x), x.size(0),
+           rowptr.numel() - 1, col_t.numel(), F, *pargs, it, _vdt(x), _stream())
+    return grad_x
+
+
 def scatter_coo(src: Tensor, index: Tensor, n_rows: int, reduce: str = "sum") -> Tensor:
     """Atomic COO fallback for an unsorted index; fp32, src: [E, F]."""
     _cuda(src, index)

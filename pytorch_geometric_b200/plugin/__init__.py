@@ -5,7 +5,7 @@ The reference has no FFI; it late-binds Python callables and a handful of option
 
   (1) functions     torch_geometric.utils.{scatter, segment, softmax, spmm} and every module that imported them by
                     name (64 modules), `edge_index._spmm` (EdgeIndex.matmul / `@`), `Aggregation.reduce`,
-                    `FusedAggregation.forward`                                             -> routing.py
+                    `FusedAggregation.forward`, `QuantileAggregation.forward`               -> routing.py
   (2) the gather    `MessagePassing._index_select` (what `_collect` / `_lift` call) returns a lazy row view, so a
                     layer whose message is `x_j` or `w * x_j` runs ONE fused CSR gather-reduce            -> lazy.py
   (3) extensions    the exact `torch_scatter` / `pyg_lib.ops` / `torch.ops.torch_sparse` operator signatures the
@@ -100,6 +100,11 @@ def install(layers: bool = False, extensions: bool = True, flip_flags: bool = Fa
 
     _set(TheirFused, "forward", fused_forward)
     counts["fused_aggregation"] = 1
+
+    # QuantileAggregation.forward (nn/aggr/quantile.py:71-131), which MedianAggregation inherits
+    from torch_geometric.nn.aggr.quantile import QuantileAggregation as TheirQuantile
+    _set(TheirQuantile, "forward", routing.make_quantile_forward(TheirQuantile.forward))
+    counts["quantile_aggregation"] = 1
 
     if extensions:
         from . import library

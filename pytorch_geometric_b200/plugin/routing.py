@@ -233,6 +233,53 @@ def make_aggr_reduce(theirs):
     return reduce
 
 
+# ------------------------------------------------------------------------------------------------ QuantileAggregation
+def make_quantile_forward(theirs):
+    """QuantileAggregation.forward (nn/aggr/quantile.py:71-131; MedianAggregation inherits it): CUDA float32 / bfloat16
+    messages with a float32 `q` buffer take one selection sweep (functional.quantile_aggregate) instead of two sorts
+    of the [E, F] matrix.  A lazy `x_j` without a scale is never gathered: its CSR comes from the layer's index pair,
+    as in fused_lazy_reduce.  A scaled one (`w * x_j`) is materialised and read as edge rows.  Everything else --
+    CPU tensors, other dtypes, compiling or scripting, no index -- runs the reference's forward."""
+    def forward(self, x, index: Optional[Tensor] = None, ptr: Optional[Tensor] = None, dim_size: Optional[int] = None,
+                dim: int = -2) -> Tensor:
+        from ..nn.aggr import quantile_layout
+        lazy = isinstance(x, LazyRows) and not isinstance(x, GatedRows)
+        src = x._src if lazy else x
+        d = dim + x.dim() if dim < 0 else dim
+        if (index is None or not engine_ok(src) or _compiling() or torch.jit.is_scripting()
+                or not isinstance(self.q, Tensor) or self.q.dtype != torch.float32 or self.q.device != src.device
+                or self.interpolation not in ops.QUANTILE_INTERPOLATIONS or (lazy and x._add is not None)):
+            if isinstance(x, LazyRows):
+                x = x.materialise()
+            return theirs(self, x, index, ptr, dim_size, dim)
+        index = _plain(index)
+        if dim_size is None:
+            dim_size = int(index.max()) + 1 if index.numel() > 0 else 0        # the reference's bincount length
+        if lazy and d == 0 and x._scale is None:
+            g = graphs.graph_from_pair(x._index, index, src.size(0), int(dim_size), ptr=None if ptr is None else _plain(ptr))
+            out = Fn.quantile_aggregate(g, src.reshape(src.size(0), -1), None, self.q, self.interpolation,
+                                        self.fill_value)
+            return quantile_layout(out, self.q.numel(), tuple(x.shape), 0)
+        if isinstance(x, LazyRows):
+            x = x.materialise()
+        xm = x.movedim(d, 0)
+        x2 = xm.reshape(xm.size(0), -1)
+        if x2.size(0) == 0:
+            return theirs(self, x, index, ptr, dim_size, dim)
+        sptr = _sorted_ptr(index, dim_size)
+        if sptr is not None:
+            out = Fn.quantile_aggregate((sptr, ops.segment_plan(sptr, x2.size(0))), None, x2, self.q,
+                                        self.interpolation, self.fill_value)
+        else:
+            e = torch.arange(index.numel(), device=index.device, dtype=index.dtype)
+            out = Fn.quantile_aggregate(CSRGraph(e, index, index.numel(), int(dim_size)), None, x2, self.q,
+                                        self.interpolation, self.fill_value)
+        return quantile_layout(out, self.q.numel(), tuple(x.shape), d)
+    forward.__wrapped__ = theirs
+    forward.__name__, forward.__doc__ = "forward", theirs.__doc__
+    return forward
+
+
 # ------------------------------------------------------------------------------------------------ MessagePassing._index_select
 def make_index_select(theirs):
     """nn/conv/message_passing.py:263-267: the gather of `_collect` / `_lift` becomes lazy (see lazy.py)."""

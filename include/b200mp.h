@@ -463,6 +463,34 @@ int b200mp_quantile_backward_src(const void* rowptr, const void* rowptr_t, const
                                  int64_t plan_n_long, int64_t plan_n_chunks, int64_t plan_chunk, float* plan_partials,
                                  int idx_dtype, int val_dtype, void* stream);
 
+/* ------------------------------------------------------------------ NNConv / ECConv (edge-conditioned message)
+ * Replaces: NNConv.message + aggregate (nn/conv/nn_conv.py:96-122: the edge network's [E, F_in F_out] output viewed as
+ * one F_in x F_out matrix per edge, a batched x_j product into [E, F_out], then scatter).  With the edge network's last
+ * Linear split off, h [E, K] (the output of everything before it, in the CALLER's edge order, read through perm; NULL
+ * perm: the slot) and h~_e = [h_e, 1], the sweep writes for destination rows [row_begin, row_end) of the CSR
+ *   P[i - row_begin, k F_in + a] = sum_{e = (j -> i)} h~_e[k] x[j, a]     (fp32; mean: / max(deg_i, 1))
+ * and out = P W' with W' [(K+1) F_in, F_out] from the last Linear's weight and bias is the caller's GEMM.  Rows
+ * without edges give 0.  Supported: K >= 0, F_in >= 1, (K + 1) F_in <= 16384 (dP_i of 64 KiB in shared memory in the
+ * backward); else B200MP_ERR_UNSUPPORTED.  reduce: SUM or MEAN.  plan_*: the destination CSR's long-row plan, partials
+ * [plan_n_chunks, (K+1) F_in] fp32 folded in chunk order (chunks of rows outside the range are skipped). */
+int b200mp_nn_conv_supported(int64_t k, int64_t fin, int val_dtype);
+int b200mp_nn_conv_csr(const void* rowptr, const void* col, const void* perm, const void* x, const void* h, float* p,
+                       int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t k, int64_t fin, int64_t row_begin,
+                       int64_t row_end, int reduce, const int64_t* plan_rows, const int64_t* plan_chunk_ptr,
+                       int64_t plan_n_long, int64_t plan_n_chunks, int64_t plan_chunk, float* plan_partials,
+                       int idx_dtype, int val_dtype, void* stream);
+/* The destination half of the backward (nn_conv.py:119-122 under autograd) for rows [row_begin, row_end): grad_p =
+ * dL/dP of those rows, fp32 in P's layout (the caller's G W'^T).  Per edge e = (j -> i), in the caller's order:
+ *   grad_h[e, k] = sum_a x[j, a] grad_p[i, k F_in + a]  (k < K)      q[e, a] = sum_{k <= K} h~_e[k] grad_p[i, k F_in + a]
+ * each divided by max(deg_i, 1) for mean and rounded once to the value dtype.  grad_h or q may be NULL (not written).
+ * grad_x is the segment sum of q's rows over the transposed CSR (b200mp_spmm_csr with perm_t as the column).
+ * plan_*: the destination CSR's plan (hub rows split into chunks; no partials: no combine step). */
+int b200mp_nn_conv_backward_dst(const void* rowptr, const void* col, const void* perm, const void* x, const void* h,
+                                const float* grad_p, void* grad_h, void* q, int64_t n_rows, int64_t n_cols,
+                                int64_t n_edges, int64_t k, int64_t fin, int64_t row_begin, int64_t row_end, int reduce,
+                                const int64_t* plan_rows, const int64_t* plan_chunk_ptr, int64_t plan_n_long,
+                                int64_t plan_n_chunks, int64_t plan_chunk, int idx_dtype, int val_dtype, void* stream);
+
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)
  * out[index[e], :] (+)= src[e, :] for an UNSORTED index.  Replaces utils/_scatter.py:14-138
  * (aten::scatter_add_ / scatter_reduce_, torch_scatter.scatter).  fp32 only.  `count` is a

@@ -13,7 +13,7 @@ from typing import Optional
 import torch
 from torch import Tensor
 
-from . import ops
+from . import dense, ops
 from .graph import CSRGraph
 
 
@@ -294,6 +294,85 @@ def aggregate_cg_uv(graph: CSRGraph, uv: Tensor, c: Optional[Tensor] = None, red
         raise ValueError(f"aggregate_cg_uv needs as many sources as destinations, got {graph.num_src} and {graph.num_dst}")
     return _AggregateCG.apply(uv.contiguous(), None, None if c is None else c.contiguous(), graph,
                               "mean" if reduce == "mean" else "sum")
+
+
+NN_CONV_BLOCK_BYTES = 1 << 29     # fp32 bytes of P = [rows, (K+1) F_in] held at once by nn_conv_aggregate
+
+
+def _nn_conv_blocks(n_dst: int, width: int):
+    """Destination row ranges [r0, r1) whose P fits NN_CONV_BLOCK_BYTES (at least one row each)."""
+    rows = max(1, NN_CONV_BLOCK_BYTES // (4 * width))
+    return [(r0, min(r0 + rows, n_dst)) for r0 in range(0, n_dst, rows)]
+
+
+class _NNConvAggregate(torch.autograd.Function):
+    """out = P W' by destination-row blocks, P_i = REDUCE_e [h_e, 1] (x) x_j (csrc/nn_conv.cu).  Nothing of size
+    N (K+1) F_in is saved: the backward recomputes each block's P for dW' = sum_b P_b^T G_b, forms dP_b = G_b W'^T for
+    the destination sweep (grad_h and q per edge), and grad_x is one segment sum of q over the transposed CSR.  Each
+    step runs only when one of its outputs is needed.  P, W' and the GEMMs are fp32; the output has x's dtype."""
+
+    @staticmethod
+    def forward(ctx, x: Tensor, h: Tensor, w_prime: Tensor, graph: CSRGraph, reduce: str):
+        width = w_prime.size(0)
+        w = w_prime.detach().float().contiguous()
+        out = torch.zeros(graph.num_dst, w.size(1), dtype=torch.float32, device=x.device)
+        for r0, r1 in _nn_conv_blocks(graph.num_dst, width):
+            p = ops.nn_conv_csr(graph.rowptr, graph.col, graph.perm, x, h, r0, r1, reduce, graph.plan)
+            out[r0:r1] = dense._mm(p, w)
+        ctx.graph, ctx.reduce = graph, reduce
+        ctx.save_for_backward(x, h, w_prime)
+        return out.to(x.dtype)
+
+    @staticmethod
+    def backward(ctx, grad_out: Tensor):
+        x, h, w_prime = ctx.saved_tensors
+        graph, reduce = ctx.graph, ctx.reduce
+        need_x, need_h, need_w = ctx.needs_input_grad[:3]
+        w = w_prime.detach().float().contiguous()
+        g = grad_out.float().contiguous()
+        E, K, Fi = graph.num_edges, h.size(1), x.size(1)
+        gh = torch.empty(E, K, dtype=x.dtype, device=x.device) if need_h else None
+        q = torch.empty(E, Fi, dtype=x.dtype, device=x.device) if need_x else None
+        gw = None
+        for r0, r1 in _nn_conv_blocks(graph.num_dst, w.size(0)):
+            g_b = g[r0:r1]
+            if need_w:
+                p = ops.nn_conv_csr(graph.rowptr, graph.col, graph.perm, x, h, r0, r1, reduce, graph.plan)
+                part = dense._mm_tn(p, g_b)
+                gw = part if gw is None else gw + part
+                del p
+            if need_x or need_h:
+                dp = dense._mm_nt(g_b, w).contiguous()
+                ops.nn_conv_backward_dst(graph.rowptr, graph.col, graph.perm, x, h, dp, r0, r1, gh, q, reduce, graph.plan)
+        if need_w and gw is None:
+            gw = torch.zeros_like(w)
+        gx = None
+        if need_x:
+            graph.build_transpose()
+            # grad_x[j] = the sum of q over j's out-edges: perm_t is the caller's edge id of each transposed slot
+            gx = ops.spmm_csr(graph.rowptr_t, graph.perm_t, None, q, graph.num_src, "sum", graph.plan_t)
+        return gx, gh, (gw.to(w_prime.dtype) if need_w else None), None, None
+
+
+def nn_conv_aggregate(graph: CSRGraph, x_src: Tensor, h: Tensor, w_prime: Tensor, reduce: str = "sum") -> Tensor:
+    """out[i] = REDUCE_{e = (j -> i)} x[j] @ reshape(h_e W2^T + b2, [F_in, F_out]) for reduce in {sum, mean}: NNConv's
+    message and aggregation (nn_conv.py:96-122) without its [E, F_in F_out] edge weights.  h: [E, K], the edge network's
+    output before its last Linear, in the caller's edge order; w_prime: [(K+1) F_in, F_out] from that Linear
+    (`nn.conv.nn_conv_weight`).  x_src: [num_src, F_in] of h's dtype; all three may require grad.  Destination rows are
+    processed in blocks whose fp32 P stays under NN_CONV_BLOCK_BYTES; a block never splits a row."""
+    if reduce not in ("sum", "add", "mean"):
+        raise ValueError(f"nn_conv_aggregate reduces by sum or mean, got '{reduce}'")
+    if x_src.dim() != 2 or x_src.size(0) != graph.num_src:
+        raise ValueError(f"x_src must be a [{graph.num_src}, F_in] tensor, got {tuple(x_src.shape)}")
+    if h.dim() != 2 or h.size(0) != graph.num_edges or h.dtype != x_src.dtype:
+        raise ValueError(f"h must be a [{graph.num_edges}, K] tensor of x's dtype, got {tuple(h.shape)} {h.dtype}")
+    K, Fi = h.size(1), x_src.size(1)
+    if w_prime.dim() != 2 or w_prime.size(0) != (K + 1) * Fi:
+        raise ValueError(f"w_prime must be a [{(K + 1) * Fi}, F_out] tensor, got {tuple(w_prime.shape)}")
+    if not ops.nn_conv_supported(K, Fi, x_src.dtype):
+        raise ValueError(f"nn_conv_aggregate does not take K = {K}, F_in = {Fi} in {x_src.dtype}")
+    return _NNConvAggregate.apply(x_src.contiguous(), h.contiguous(), w_prime, graph,
+                                  "mean" if reduce == "mean" else "sum")
 
 
 def _param_aggr_operands(graph, x: Optional[Tensor], a: Optional[Tensor], w, name: str, what: str):

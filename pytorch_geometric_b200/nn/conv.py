@@ -14,6 +14,7 @@ Two layers of code:
       GINEConv        nn/conv/gin_conv.py:104-207        nn.*, eps [1], lin.weight/bias (edge_dim)
       ResGatedGraphConv nn/conv/res_gated_graph_conv.py:13-148  lin_key/lin_query/lin_value.weight/bias, lin_skip.weight, bias
       CGConv          nn/conv/cg_conv.py:12-101          lin_f.weight/bias, lin_s.weight/bias, bn.* (batch_norm)
+      NNConv          nn/conv/nn_conv.py:13-126          nn.*, lin.weight (root_weight), bias
       GENConv         nn/conv/gen_conv.py:45-243         aggr_module.t/p, lin_src/lin_edge/lin_dst.weight, mlp.*, msg_norm.scale
       PNAConv         nn/conv/pna_conv.py:20-209         aggr_module.avg_deg_lin/log, edge_encoder.*, pre_nns.t.0.*, post_nns.*, lin.*
       RGCNConv        nn/conv/rgcn_conv.py:40-300        weight [R,in,out] (or bases/blocks + comp), root, bias
@@ -607,6 +608,108 @@ class CGConv(torch.nn.Module):
 
     def __repr__(self) -> str:
         return f"{self.__class__.__name__}({self.channels}, dim={self.dim})"
+
+
+def _plain_linear(m) -> bool:
+    t = type(m)
+    return t is torch.nn.Linear or (t.__name__ == "Linear" and t.__module__ == "torch_geometric.nn.dense.linear")
+
+
+def _module_hooks(m) -> bool:
+    return bool(m._forward_hooks or m._forward_pre_hooks or m._backward_hooks or m._backward_pre_hooks)
+
+
+def _global_module_hooks() -> bool:
+    from torch.nn.modules import module as M
+    return bool(M._global_forward_hooks or M._global_forward_pre_hooks or M._global_backward_hooks
+                or M._global_backward_pre_hooks)
+
+
+def nn_conv_split(net, f_in: int, f_out: int):
+    """(modules before the last Linear, the last Linear) of NNConv's edge network, or None where it cannot be split:
+    the network must be a `torch.nn.Linear` / `torch_geometric.nn.Linear`, or a `torch.nn.Sequential` ending in one,
+    whose weight is initialised (not lazy) with F_in F_out rows.  The fused path never calls the network itself nor its
+    last Linear, so any forward or backward hook on either, and any global module hook, makes it unsplittable: the
+    reference would fire them."""
+    mods = list(net) if type(net) is torch.nn.Sequential else [net]
+    if not mods or not _plain_linear(mods[-1]):
+        return None
+    last = mods[-1]
+    w = last.weight
+    if isinstance(w, torch.nn.parameter.UninitializedParameter) or w.dim() != 2 or w.size(0) != f_in * f_out:
+        return None
+    if _module_hooks(net) or _module_hooks(last) or _global_module_hooks():
+        return None
+    return mods[:-1], last
+
+
+def nn_conv_weight(w2: Tensor, b2: Optional[Tensor], f_in: int, f_out: int) -> Tensor:
+    """W' [(K+1) F_in, F_out] of NNConv's last edge-network Linear (weight w2 [F_in F_out, K], bias b2): row k F_in + a
+    holds W2.view(F_in, F_out, K)[a, :, k] and the last F_in rows b2.view(F_in, F_out), so that
+    out_i = vec(P_i) W' with P_i = sum_e [h_e, 1] (x) x_j (nn_conv.py:119-122).  Views and a cat of the parameters, so
+    autograd maps dW' back to w2 and b2."""
+    K = w2.size(1)
+    wp = w2.view(f_in, f_out, K).permute(2, 0, 1)
+    bp = b2.view(1, f_in, f_out) if b2 is not None else w2.new_zeros(1, f_in, f_out)
+    return torch.cat([wp, bp], dim=0).reshape((K + 1) * f_in, f_out)
+
+
+def nn_conv_edge_hidden(pre, edge_attr: Tensor) -> Tensor:
+    """The edge network's output before its last Linear: the user's own modules, run as torch runs them."""
+    h = edge_attr
+    for m in pre:
+        h = m(h)
+    return h
+
+
+class NNConv(torch.nn.Module):
+    """x_i Theta + AGGR_j x_j h(e_ji) + bias (nn_conv.py:13-126) with AGGR = sum (default) or mean.  The edge network
+    h must end in a Linear (`nn_conv_split`); everything before it runs as torch modules, and the message runs with its
+    aggregation as one sweep into P plus one GEMM (`Fn.nn_conv_aggregate`), without the [E, F_in F_out] weights.  Other
+    aggregations and edge networks raise ValueError."""
+
+    def __init__(self, in_channels, out_channels: int, nn, aggr: str = "add", root_weight: bool = True,
+                 bias: bool = True, **kwargs):
+        super().__init__()
+        if aggr not in ("add", "sum", "mean"):
+            raise ValueError(f"aggr='{aggr}' is not on the fused path (add, sum or mean)")
+        ch = (in_channels, in_channels) if isinstance(in_channels, int) else tuple(in_channels)
+        if nn_conv_split(nn, ch[0], out_channels) is None:
+            raise ValueError("the edge network must be a Linear, or a torch.nn.Sequential ending in one, with "
+                             f"{ch[0]} * {out_channels} = {ch[0] * out_channels} initialised output features")
+        self.in_channels, self.out_channels, self.aggr = in_channels, out_channels, aggr
+        self.nn = nn
+        self.root_weight = root_weight
+        self.in_channels_l = ch[0]
+        self.flow = kwargs.get("flow", "source_to_target")
+        if root_weight:
+            self.lin = _Lin(ch[1], out_channels, bias=False)                          # nn_conv.py:79-81
+            bound = 1.0 / math.sqrt(ch[1])
+            with torch.no_grad():
+                self.lin.weight.uniform_(-bound, bound)
+        self.bias = torch.nn.Parameter(torch.zeros(out_channels)) if bias else None
+
+    def forward(self, x, edge_index: Adj, edge_attr: Tensor, size=None) -> Tensor:
+        pair = _pair(x)
+        split = nn_conv_split(self.nn, self.in_channels_l, self.out_channels)
+        if split is None:
+            raise ValueError("the edge network can no longer be split at its last Linear (a hook on it or on that "
+                             "Linear, a global module hook, or a changed Linear); NNConv has no unfused path")
+        if torch.is_autocast_enabled(pair[0].device.type):
+            raise ValueError("NNConv runs in the dtype of its inputs; it does not run under torch.autocast")
+        graph = _plain_graph(edge_index, pair[0].size(0), _num_dst(pair, size), self.flow)
+        pre, last = split
+        w_prime = nn_conv_weight(last.weight, last.bias, self.in_channels_l, self.out_channels)
+        out = Fn.nn_conv_aggregate(graph, pair[0], nn_conv_edge_hidden(pre, edge_attr), w_prime,
+                                   "mean" if self.aggr == "mean" else "sum")
+        if pair[1] is not None and self.root_weight:                                   # nn_conv.py:110-115
+            out = out + self.lin(pair[1])
+        if self.bias is not None:
+            out = out + self.bias
+        return out
+
+    def __repr__(self) -> str:
+        return f"{self.__class__.__name__}({self.in_channels}, {self.out_channels}, aggr={self.aggr}, nn={self.nn})"
 
 
 def pna_uv_c(x: Tensor, edge_attr: Optional[Tensor], pre_weights, pre_biases, enc_w: Optional[Tensor],

@@ -575,6 +575,64 @@ def cg_backward_src(rowptr_t: Tensor, col_t: Tensor, perm_t: Tensor, val_t: Opti
     return grad_v
 
 
+def nn_conv_supported(k: int, f_in: int, dtype: torch.dtype) -> bool:
+    """Whether the NNConv sweeps take K hidden edge features and F_in source channels in this dtype."""
+    if dtype not in (torch.float32, torch.bfloat16):
+        return False
+    return bool(lib().b200mp_nn_conv_supported(int(k), int(f_in), F32 if dtype == torch.float32 else BF16))
+
+
+def _nn_conv_operands(col: Tensor, x: Tensor, h: Tensor):
+    if x.dim() != 2 or h.dim() != 2 or h.size(0) != col.numel() or h.dtype != x.dtype:
+        raise ValueError(f"x must be [n_src, F_in] and h [{col.numel()}, K] of x's dtype, got {tuple(x.shape)} "
+                         f"{x.dtype} and {tuple(h.shape)} {h.dtype}")
+    return x.contiguous(), h.contiguous(), h.size(1), x.size(1)
+
+
+def nn_conv_csr(rowptr: Tensor, col: Tensor, perm: Optional[Tensor], x: Tensor, h: Tensor, row_begin: int, row_end: int,
+                reduce: str = "sum", plan: Optional[LongRowPlan] = None) -> Tensor:
+    """P [row_end - row_begin, (K+1) F_in] fp32 with P[i, k F_in + a] = REDUCE_{e in row i} [h[perm[e]], 1][k] x[col[e], a]
+    for sum / mean: NNConv's message with the edge network's last Linear split off (out = P W').  h: [E, K] in the
+    caller's edge order; perm: CSR slot -> caller's edge id, None for an adopted CSR."""
+    _cuda(rowptr, col, perm, x, h)
+    if reduce not in ("sum", "add", "mean"):
+        raise ValueError(f"nn_conv_csr reduces by sum or mean, not '{reduce}'")
+    x, h, K, Fi = _nn_conv_operands(col, x, h)
+    it = _same_idx(rowptr, col, perm)
+    width = (K + 1) * Fi
+    p = torch.empty(row_end - row_begin, width, dtype=torch.float32, device=x.device)
+    # the hub chunks' partials, n_chunks * (K+1) F_in fp32, live for this call only: a [n_chunks, 16384] buffer cached on
+    # the plan would stay with the graph
+    part = None if plan is None or not plan.n_long else \
+        torch.empty(plan.n_chunks * width, dtype=torch.float32, device=x.device)
+    pargs = (*_plan_rows(plan), _p(part))
+    _timed("nn_conv_csr", 2 if pargs[2] else 1, lib().b200mp_nn_conv_csr, _p(rowptr), _p(col), _p(perm), _p(x), _p(h),
+           _p(p), rowptr.numel() - 1, x.size(0), col.numel(), K, Fi, int(row_begin), int(row_end), REDUCE[reduce], *pargs,
+           it, _vdt(x), _stream())
+    return p
+
+
+def nn_conv_backward_dst(rowptr: Tensor, col: Tensor, perm: Optional[Tensor], x: Tensor, h: Tensor, grad_p: Tensor,
+                         row_begin: int, row_end: int, grad_h: Optional[Tensor], q: Optional[Tensor], reduce: str = "sum",
+                         plan: Optional[LongRowPlan] = None) -> None:
+    """Destination sweep of NNConv's backward for rows [row_begin, row_end): writes, per edge in the caller's order,
+    grad_h[e, k] = x_j . grad_p[i, k, :] into `grad_h` ([E, K]) and q[e, :] = h~_e . grad_p[i] into `q` ([E, F_in]),
+    either of them None to skip it.  grad_p: fp32 [row_end - row_begin, (K+1) F_in]."""
+    _cuda(rowptr, col, perm, x, h, grad_p, grad_h, q)
+    x, h, K, Fi = _nn_conv_operands(col, x, h)
+    E = col.numel()
+    if tuple(grad_p.shape) != (row_end - row_begin, (K + 1) * Fi) or grad_p.dtype != torch.float32 \
+            or not grad_p.is_contiguous():
+        raise ValueError(f"grad_p must be a contiguous fp32 [{row_end - row_begin}, {(K + 1) * Fi}] tensor")
+    for name, t, w in (("grad_h", grad_h, K), ("q", q, Fi)):
+        if t is not None and (tuple(t.shape) != (E, w) or t.dtype != x.dtype or not t.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous [{E}, {w}] tensor of x's dtype")
+    it = _same_idx(rowptr, col, perm)
+    _timed("nn_conv_backward_dst", 1, lib().b200mp_nn_conv_backward_dst, _p(rowptr), _p(col), _p(perm), _p(x), _p(h),
+           _p(grad_p), _p(grad_h), _p(q), rowptr.numel() - 1, x.size(0), E, K, Fi, int(row_begin), int(row_end),
+           REDUCE[reduce], *_plan_rows(plan), it, _vdt(x), _stream())
+
+
 SOFTMAX_MESSAGES = {"identity": 0, "relu_eps": 1}
 
 

@@ -26,6 +26,7 @@ from torch_geometric.typing import (Adj, NoneType, OptPairTensor, OptTensor, Pai
 
 from .. import dense
 from .. import functional as Fn
+from .. import ops
 from .. import utils as U
 from ..graph import CSRGraph, cached_graph
 from ..nn import conv as C
@@ -36,7 +37,8 @@ from ._util import plain
 # Inspector caches class sources by `cls.__name__` (torch_geometric/inspector.py:323-334), so a subclass that reused
 # its parent's name would hide the parent's `# propagate_type:` annotation and get a `propagate` without arguments.
 LAYERS = {n: "B200" + n for n in ("GCNConv", "SAGEConv", "GraphConv", "GINConv", "GATConv", "GATv2Conv", "TransformerConv",
-                                  "RGCNConv", "FastRGCNConv", "PNAConv", "CGConv", "GENConv")}
+                                  "RGCNConv", "FastRGCNConv", "PNAConv", "CGConv", "GENConv", "NNConv")}
+LAYERS["ECConv"] = "B200NNConv"                 # the reference's alias of NNConv (nn/conv/__init__.py)
 
 
 def _has_hooks(self) -> bool:
@@ -405,4 +407,47 @@ class B200GENConv(tgnn.GENConv):
                         x_dst = self.lin_dst(x_dst)
                     out = out + x_dst
                 return self.mlp(out)
+        return super().forward(x, edge_index, edge_attr, size)
+
+
+def _nn_conv_split(self, xs, edge_index, edge_attr):
+    """The split edge network (`C.nn_conv_split`) when the fused NNConv path covers the call, else None: sum / mean
+    aggregation, a splittable edge network, a 2-D edge_attr, a [2, E] tensor or EdgeIndex adjacency, CUDA float32 /
+    bfloat16 tensors and parameters of one dtype outside torch.autocast (which would run the edge network, and so h,
+    in another dtype than x), and a shape the sweeps take."""
+    if type(self.aggr_module) not in (tgnn.aggr.SumAggregation, tgnn.aggr.MeanAggregation):
+        return None
+    if xs[0] is not None and torch.is_autocast_enabled(xs[0].device.type):
+        return None
+    if xs[0] is None or xs[0].dim() != 2 or xs[0].size(1) != self.in_channels_l or edge_attr is None or edge_attr.dim() != 2:
+        return None
+    if not (isinstance(edge_index, Tensor) and edge_index.layout == torch.strided and edge_index.dim() == 2
+            and edge_index.size(0) == 2 and not edge_index.is_floating_point()):
+        return None
+    split = C.nn_conv_split(self.nn, self.in_channels_l, self.out_channels)
+    if split is None:
+        return None
+    ts = [t for t in (xs[0], xs[1], edge_attr) if t is not None]
+    if not _fast(self, *ts) or len({t.dtype for t in ts} | {p.dtype for p in self.parameters()}) != 1:
+        return None
+    return split if ops.nn_conv_supported(split[1].weight.size(1), self.in_channels_l, xs[0].dtype) else None
+
+
+class B200NNConv(tgnn.NNConv):
+    def forward(self, x, edge_index, edge_attr=None, size=None) -> Tensor:
+        xs = _pair(x)
+        split = _nn_conv_split(self, xs, edge_index, edge_attr)
+        if split is not None:
+            g = _graph(edge_index, xs[0].size(0), _ndst(xs, size), self.flow)
+            if g is not None:
+                pre, last = split
+                h = C.nn_conv_edge_hidden(pre, edge_attr)
+                w_prime = C.nn_conv_weight(last.weight, last.bias, self.in_channels_l, self.out_channels)
+                reduce = "mean" if type(self.aggr_module) is tgnn.aggr.MeanAggregation else "sum"
+                out = Fn.nn_conv_aggregate(g, xs[0], h, w_prime, reduce)
+                if xs[1] is not None and self.root_weight:                             # nn_conv.py:110-115
+                    out = out + self.lin(xs[1])
+                if self.bias is not None:
+                    out = out + self.bias
+                return out
         return super().forward(x, edge_index, edge_attr, size)

@@ -160,6 +160,23 @@ int b200mp_spmm_csr(const void* rowptr, const void* col, const float* val, const
                     const void* x_halo, int64_t n_local_cols, int flags, const void* peer_ptrs,
                     int64_t peer_rows, const void* relu_mask, int idx_dtype, int val_dtype, void* stream);
 
+/* The transposed sweep of GCNConv's backward with its bias gradient: b200mp_spmm_csr's weighted sum over the
+ * transposed CSR (rowptr_t, col_t, val_t; reduce sum, val_t required; no bias, halo, peer table, accumulate or
+ * relu_mask), out[j, :] = sum_e val_t[e] * x[col_t[e], :], that also returns colsum_out[f] = sum_i x[i, f] in fp32.
+ * It needs a square graph in which every row i holds exactly one edge with col_t == i (GCN's self-loops, which the
+ * CSR and its transpose both have): the sweep adds the x row of that edge, already loaded for the sum, so the column
+ * sum costs no second read of x.  out is bit-identical to b200mp_spmm_csr's.  x: [n_rows, feat].  Long rows: the
+ * transposed CSR's plan (long_rows_t, chunk_ptr_t, n_long_rows_t, n_chunks_t, chunk) and partials_t as in
+ * b200mp_spmm_csr.  colsum_parts: caller-owned fp32 workspace [n_parts, feat]: one row per CTA of the sweep (a grid
+ * of resident CTAs, 8 per SM) and, behind them, the second level of the fold (b200mp_column_sum); pass 16 * #SMs.  The
+ * column sum is deterministic on a given device.  Rows that are not whole 16-byte vectors, and rows so wide (above 3072
+ * values) that the per-warp column slots pass 48 KB of shared memory, take the plain sweep and b200mp_column_sum. */
+int b200mp_spmm_csr_self_colsum(const void* rowptr_t, const void* col_t, const float* val_t, const void* x, void* out,
+                                float* colsum_out, int64_t n_rows, int64_t feat, const int64_t* long_rows_t,
+                                const int64_t* chunk_ptr_t, int64_t n_long_rows_t, int64_t n_chunks_t, int64_t chunk,
+                                float* partials_t, float* colsum_parts, int64_t n_parts, int idx_dtype, int val_dtype,
+                                void* stream);
+
 /* Segmented reduce without gather: out[i,:] = REDUCE_{e in [ptr[i], ptr[i+1])} src[e,:].
  * Replaces utils/_segment.py:11-50 (torch._segment_reduce / torch_scatter.segment_csr) and the
  * sorted-index case of utils/_scatter.py:14-138.  Same empty-segment and +-inf -> 0 rules.

@@ -39,6 +39,8 @@ _SIGS = {
     "b200mp_csr_plan_fill": (_INT, [_P, _I64, _I64, _I64, _P, _P, _P, _I64, _INT, _P]),
     "b200mp_spmm_csr": (_INT, [_P, _P, _P, _P, _P, _I64, _I64, _I64, _INT, _P, _P, _I64, _I64, _I64, _P,
                                _P, _P, _I64, _INT, _P, _I64, _P, _INT, _INT, _P]),
+    "b200mp_spmm_csr_self_colsum": (_INT, [_P, _P, _P, _P, _P, _P, _I64, _I64, _P, _P, _I64, _I64, _I64, _P, _P, _I64,
+                                           _INT, _INT, _P]),
     "b200mp_segment_csr": (_INT, [_P, _P, _P, _I64, _I64, _I64, _INT, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
     "b200mp_minmax_ties": (_INT, [_P, _P, _P, _P, _P, _P, _I64, _I64, _INT, _INT, _INT, _P]),
     "b200mp_minmax_backward": (_INT, [_P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _INT, _INT, _P]),

@@ -146,6 +146,41 @@ extern "C" int b200mp_spmm_csr(const void* rowptr, const void* col, const float*
     });
 }
 
+extern "C" int b200mp_spmm_csr_self_colsum(const void* rowptr_t, const void* col_t, const float* val_t, const void* x,
+                                           void* out, float* colsum_out, int64_t n_rows, int64_t feat,
+                                           const int64_t* long_rows_t, const int64_t* chunk_ptr_t, int64_t n_long_rows_t,
+                                           int64_t n_chunks_t, int64_t chunk, float* partials_t, float* colsum_parts,
+                                           int64_t n_parts, int idx_dtype, int val_dtype, void* stream) {
+    B200MP_CHECK_ARG(n_rows >= 0 && feat >= 0 && n_parts >= 1);
+    LongRowPlan plan;
+    if (int rc = make_plan(plan, long_rows_t, chunk_ptr_t, n_long_rows_t, n_chunks_t, chunk, partials_t, true)) return rc;
+    if (feat == 0) return B200MP_OK;
+    B200MP_CHECK_ARG(colsum_out && colsum_parts);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (n_rows == 0) return b200mp_column_sum(nullptr, colsum_out, colsum_parts, 1, 0, feat, val_dtype, stream);
+    B200MP_CHECK_ARG(rowptr_t && col_t && val_t && x && out);
+    return dispatch_val_idx(val_dtype, idx_dtype, "spmm_csr_self_colsum", [&](auto tv, auto ti) {
+        using T = decltype(tv);
+        using I = decltype(ti);
+        int64_t parts = 0;
+        if (int rc = csr_sum_self_colsum<T, I>(static_cast<const I*>(rowptr_t), static_cast<const I*>(col_t), val_t,
+                                               static_cast<const T*>(x), static_cast<T*>(out), n_rows, feat, plan,
+                                               colsum_parts, n_parts - ceil_div(n_parts, 64), parts, s))
+            return rc;
+        // the per-CTA partials are a [parts, feat] fp32 matrix: fold them by the column sum, its second level behind them
+        if (parts > 0)
+            return b200mp_column_sum(colsum_parts, colsum_out, colsum_parts + parts * feat, b200mp_column_sum_parts(parts),
+                                     parts, feat, B200MP_F32, stream);
+        // no vector kernel for this row shape: the plain sweep, then a column sum of x (one row per self-loop)
+        if (int rc = csr_reduce_dispatch<T, I, B200MP_SUM, true>(static_cast<const I*>(rowptr_t), static_cast<const I*>(col_t),
+                                                                 val_t, static_cast<const T*>(x), static_cast<T*>(out),
+                                                                 n_rows, feat, false, false, plan, nullptr, s))
+            return rc;
+        return b200mp_column_sum(x, colsum_out, colsum_parts, std::min(n_parts, b200mp_column_sum_parts(n_rows)), n_rows,
+                                 feat, val_dtype, stream);
+    });
+}
+
 extern "C" int b200mp_minmax_ties(const void* rowptr, const void* col, const float* val, const void* x,
                                   const void* out, float* ties, int64_t n_rows, int64_t feat,
                                   int count_self_zero, int idx_dtype, int val_dtype, void* stream) {

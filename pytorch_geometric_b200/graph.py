@@ -23,6 +23,10 @@ _INT32_MAX = 2**31 - 1
 
 
 class CSRGraph:
+    # Every destination row i holds exactly one edge i -> i (so does every row of the transposed CSR).  Set only by
+    # utils.gcn_norm_graph with self-loops added; a graph built, adopted or narrowed any other way leaves it False.
+    one_self_loop_per_row = False
+
     def __init__(self, src: Tensor, dst: Tensor, num_src: int, num_dst: int,
                  edge_weight: Optional[Tensor] = None, chunk: int = DEFAULT_CHUNK,
                  idx_dtype: Optional[torch.dtype] = None):

@@ -84,8 +84,12 @@ class _BiasAggregate(torch.autograd.Function):
         gx = gb = None
         if ctx.needs_input_grad[0]:
             graph.build_transpose()
-            gx = ops.spmm_csr(graph.rowptr_t, graph.col_t, graph.val_t, grad_out, graph.num_src, "sum", graph.plan_t)
-        if ctx.needs_input_grad[1]:
+            if ctx.needs_input_grad[1] and graph.one_self_loop_per_row and graph.val_t is not None:
+                # row i of A^T gathers grad_out[i] once, through its self-loop: the bias gradient rides the sweep
+                gx, gb = ops.spmm_csr_self_colsum(graph.rowptr_t, graph.col_t, graph.val_t, grad_out, graph.plan_t)
+            else:
+                gx = ops.spmm_csr(graph.rowptr_t, graph.col_t, graph.val_t, grad_out, graph.num_src, "sum", graph.plan_t)
+        if ctx.needs_input_grad[1] and gb is None:
             gb = ops.column_sum(grad_out)
         return gx, gb, None
 

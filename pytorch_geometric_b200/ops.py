@@ -302,6 +302,32 @@ def spmm_csr(rowptr: Tensor, col: Tensor, val: Optional[Tensor], x: Tensor, n_ro
     return out
 
 
+def spmm_csr_self_colsum(rowptr: Tensor, col: Tensor, val: Tensor, x: Tensor,
+                         plan: Optional[LongRowPlan] = None) -> Tuple[Tensor, Tensor]:
+    """(spmm_csr(rowptr, col, val, x, N, "sum", plan), x.sum(0) in fp32) for a square graph whose every row i holds
+    exactly one edge i -> i (CSRGraph.one_self_loop_per_row): the column sum is taken from the self-loop rows the
+    sweep already loads, not from a second pass over x (b200mp_spmm_csr_self_colsum)."""
+    _cuda(rowptr, col, val, x)
+    if x.dim() != 2 or x.size(0) != rowptr.numel() - 1:
+        raise ValueError("spmm_csr_self_colsum expects a square graph and an [N, F] feature matrix")
+    x = x.contiguous()
+    it = _same_idx(rowptr, col)
+    val = val.contiguous().float()
+    n, F = x.shape
+    out = torch.empty(n, F, dtype=x.dtype, device=x.device)
+    colsum = torch.empty(F, dtype=torch.float32, device=x.device)
+    # one fp32 partial row per CTA: 16 resident 128-thread CTAs per SM at most
+    parts = 16 * torch.cuda.get_device_properties(x.device).multi_processor_count
+    ws = torch.empty(parts * max(F, 1), dtype=torch.float32, device=x.device)
+    if plan is not None and plan.n_long:
+        args = (_p(plan.long_rows), _p(plan.chunk_ptr), plan.n_long, plan.n_chunks, plan.chunk, _p(plan.partials(F, x.device)))
+    else:
+        args = (None, None, 0, 0, 0, None)
+    _timed("spmm_csr", 3 if args[2] else 2, lib().b200mp_spmm_csr_self_colsum, _p(rowptr), _p(col), _p(val), _p(x),
+           _p(out), _p(colsum), n, F, *args, _p(ws), parts, it, _vdt(x), _stream())
+    return out, colsum
+
+
 SEGMENT_PLAN_MIN_ROWS = 1 << 16   # below this many source rows a hub segment cannot matter: skip the plan (and its sync)
 SEGMENT_CHUNK = 512               # rows per chunk of a long segment (same as graph.DEFAULT_CHUNK)
 

@@ -212,6 +212,7 @@ def gcn_norm_graph(edge_index: Tensor, edge_weight: Optional[Tensor] = None, num
     src, dst = (row, col) if flow == "source_to_target" else (col, row)
     kw = {} if chunk is None else {"chunk": chunk}
     g = CSRGraph(src, dst, N, N, None, **kw)
+    g.one_self_loop_per_row = add_self_loops      # self_loops drops the graph's own loops and adds one per node
     # deg is summed over `col` for source_to_target, `row` otherwise == the aggregation target
     w_csr = None if w is None else g.to_csr_order(w.float())
     _, w_norm = ops.gcn_norm_csr(g.rowptr, g.col, w_csr)

@@ -508,6 +508,63 @@ int b200mp_nn_conv_backward_dst(const void* rowptr, const void* col, const void*
                                 const int64_t* plan_rows, const int64_t* plan_chunk_ptr, int64_t plan_n_long,
                                 int64_t plan_n_chunks, int64_t plan_chunk, int idx_dtype, int val_dtype, void* stream);
 
+/* ------------------------------------------------------------------ SplineConv (B-spline basis and weighting)
+ * Supported: degree 1..3, S = (degree + 1)^D basis slots per edge with 1 <= S <= 64; the fused sweeps also need
+ * K >= 1, F_in >= 1 and K F_in <= 16384 (P_i in shared memory); else B200MP_ERR_UNSUPPORTED.  Values fp32 or bf16. */
+int b200mp_spline_supported(int64_t k, int64_t fin, int64_t s, int val_dtype);
+/* Replaces pyg_lib.ops.spline_basis (spline_conv.py:151-152).  pseudo [E, D] (val_dtype), kernel_size [D] int64,
+ * is_open_spline [D] uint8, all on the device.  Writes basis [E, S] (val_dtype) and weight_index [E, S] (wi_dtype,
+ * B200MP_I32 or B200MP_I64): for slot s, with k_d the d-th base-(degree+1) digit of s (dimension 0 fastest) and
+ * v_d = pseudo[e, d] * (kernel_size[d] - degree * is_open_spline[d]) in fp32,
+ *   weight_index = sum_d ((floor(v_d) + k_d) mod kernel_size[d]) prod_{d' < d} kernel_size[d'],  basis = prod_d B(t_d, k_d)
+ * with t_d = v_d - floor(v_d).  The modulo is non-negative and kernel sizes below 1 count as 1, so pseudo outside
+ * [0, 1] gives indices in [0, K) (the reference leaves that case undefined). */
+int b200mp_spline_basis(const void* pseudo, const int64_t* kernel_size, const uint8_t* is_open_spline, void* basis,
+                        void* weight_index, int64_t n_edges, int64_t dim, int degree, int val_dtype, int wi_dtype,
+                        void* stream);
+/* The basis's backward (pyg_lib.ops.spline_basis under autograd): grad_pseudo [E, D] = sum_s grad_basis[e, s] d basis[e, s]
+ * / d pseudo[e, d] in fp32, in slot order, rounded once to val_dtype. */
+int b200mp_spline_basis_backward(const void* grad_basis, const void* pseudo, const int64_t* kernel_size,
+                                 const uint8_t* is_open_spline, void* grad_pseudo, int64_t n_edges, int64_t dim,
+                                 int degree, int val_dtype, void* stream);
+/* Replaces pyg_lib.ops.spline_weighting (spline_conv.py:153): out[e] = sum_s basis[e, s] x[e] @ weight[wi[e, s]] for
+ * x [E, F_in], weight [K, F_in, F_out], basis and weight_index [E, S] (idx_dtype) -- the standalone, unfused op.
+ * A slot whose index lies outside [0, K) contributes nothing. */
+int b200mp_spline_weighting(const void* x, const void* weight, const void* basis, const void* weight_index, void* out,
+                            int64_t n_edges, int64_t fin, int64_t fout, int64_t k, int64_t s, int idx_dtype,
+                            int val_dtype, void* stream);
+/* Its backward; each of grad_x [E, F_in], grad_basis [E, S] (val_dtype) and grad_weight [K, F_in, F_out] (fp32) may be
+ * NULL (not computed).  grad_weight needs slot_order (the flat slot ids e S + s sorted by weight index, stably) and
+ * slot_ptr [K + 1] (where each kernel's slots begin in it), both of idx_dtype; each kernel's slots are summed in that
+ * order. */
+int b200mp_spline_weighting_backward(const void* grad_out, const void* x, const void* weight, const void* basis,
+                                     const void* weight_index, const void* slot_order, const void* slot_ptr,
+                                     void* grad_x, void* grad_basis, float* grad_weight, int64_t n_edges, int64_t fin,
+                                     int64_t fout, int64_t k, int64_t s, int idx_dtype, int val_dtype, void* stream);
+/* Replaces SplineConv.message + aggregate (spline_conv.py:150-153 and the sum / mean scatter) for destination rows
+ * [row_begin, row_end) of the CSR: with basis [E, S] (val_dtype) and weight_index [E, S] int32 in the CALLER's edge
+ * order, read through perm (NULL: the slot),
+ *   P[i - row_begin, k F_in + a] = sum_{e = (j -> i), s : wi[e, s] = k} basis[e, s] x[j, a]   (fp32; mean: / max(deg_i, 1))
+ * and out = P weight.view(K F_in, F_out) is the caller's GEMM.  Rows without edges give 0; slots whose index lies outside
+ * [0, K) add nothing.  reduce: SUM or MEAN.  plan_*: the destination CSR's long-row plan, partials
+ * [plan_n_chunks, K F_in] fp32 folded in chunk order (chunks of rows outside the range are skipped). */
+int b200mp_spline_csr(const void* rowptr, const void* col, const void* perm, const void* x, const void* basis,
+                      const int32_t* weight_index, float* p, int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t k,
+                      int64_t fin, int64_t s, int64_t row_begin, int64_t row_end, int reduce, const int64_t* plan_rows,
+                      const int64_t* plan_chunk_ptr, int64_t plan_n_long, int64_t plan_n_chunks, int64_t plan_chunk,
+                      float* plan_partials, int idx_dtype, int val_dtype, void* stream);
+/* The destination half of its backward for rows [row_begin, row_end): grad_p = dL/dP of those rows, fp32 in P's layout
+ * (the caller's G weight^T).  Per edge e = (j -> i), in the caller's order, with dP_i divided by max(deg_i, 1) for mean:
+ *   grad_basis[e, s] = <dP_i[wi[e, s]], x[j]>        q[e, a] = sum_s basis[e, s] dP_i[wi[e, s], a]
+ * rounded once to val_dtype; either may be NULL (not written).  grad_x is the segment sum of q over the transposed CSR.
+ * plan_*: the destination CSR's plan (no partials: no combine step). */
+int b200mp_spline_backward_dst(const void* rowptr, const void* col, const void* perm, const void* x, const void* basis,
+                               const int32_t* weight_index, const float* grad_p, void* grad_basis, void* q,
+                               int64_t n_rows, int64_t n_cols, int64_t n_edges, int64_t k, int64_t fin, int64_t s,
+                               int64_t row_begin, int64_t row_end, int reduce, const int64_t* plan_rows,
+                               const int64_t* plan_chunk_ptr, int64_t plan_n_long, int64_t plan_n_chunks,
+                               int64_t plan_chunk, int idx_dtype, int val_dtype, void* stream);
+
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)
  * out[index[e], :] (+)= src[e, :] for an UNSORTED index.  Replaces utils/_scatter.py:14-138
  * (aten::scatter_add_ / scatter_reduce_, torch_scatter.scatter).  fp32 only.  `count` is a

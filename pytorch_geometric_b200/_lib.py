@@ -78,6 +78,13 @@ _SIGS = {
     "b200mp_nn_conv_supported": (_INT, [_I64, _I64, _INT]),
     "b200mp_nn_conv_csr": (_INT, [_P] * 6 + [_I64] * 7 + [_INT, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
     "b200mp_nn_conv_backward_dst": (_INT, [_P] * 8 + [_I64] * 7 + [_INT, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
+    "b200mp_spline_supported": (_INT, [_I64, _I64, _I64, _INT]),
+    "b200mp_spline_basis": (_INT, [_P] * 5 + [_I64, _I64, _INT, _INT, _INT, _P]),
+    "b200mp_spline_basis_backward": (_INT, [_P] * 5 + [_I64, _I64, _INT, _INT, _P]),
+    "b200mp_spline_weighting": (_INT, [_P] * 5 + [_I64] * 5 + [_INT, _INT, _P]),
+    "b200mp_spline_weighting_backward": (_INT, [_P] * 10 + [_I64] * 5 + [_INT, _INT, _P]),
+    "b200mp_spline_csr": (_INT, [_P] * 7 + [_I64] * 8 + [_INT, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
+    "b200mp_spline_backward_dst": (_INT, [_P] * 9 + [_I64] * 8 + [_INT, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
     "b200mp_scatter_coo": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
     "b200mp_split_tf32": (_INT, [_P, _P, _P, _I64, _P]),
     "b200mp_split_tf32_transposed": (_INT, [_P, _P, _P, _I64, _I64, _P]),

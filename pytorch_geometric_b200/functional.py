@@ -375,6 +375,142 @@ def nn_conv_aggregate(graph: CSRGraph, x_src: Tensor, h: Tensor, w_prime: Tensor
                                   "mean" if reduce == "mean" else "sum")
 
 
+class _SplineBasis(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, pseudo: Tensor, kernel_size: Tensor, is_open_spline: Tensor, degree: int, wi_dtype: torch.dtype):
+        basis, wi = ops.spline_basis(pseudo, kernel_size, is_open_spline, degree, wi_dtype)
+        ctx.degree = degree
+        ctx.save_for_backward(pseudo, kernel_size, is_open_spline)
+        ctx.mark_non_differentiable(wi)
+        return basis, wi
+
+    @staticmethod
+    def backward(ctx, grad_basis: Tensor, _grad_wi):
+        pseudo, kernel_size, is_open_spline = ctx.saved_tensors
+        gp = None
+        if ctx.needs_input_grad[0]:
+            gp = ops.spline_basis_backward(grad_basis, pseudo, kernel_size, is_open_spline, ctx.degree)
+        return gp, None, None, None, None
+
+
+def spline_basis(pseudo: Tensor, kernel_size: Tensor, is_open_spline: Tensor, degree: int = 1,
+                 wi_dtype: torch.dtype = torch.int64):
+    """(basis [E, S], weight_index [E, S]) of pyg_lib.ops.spline_basis on CUDA float32 / bfloat16 pseudo-coordinates
+    [E, D], differentiable with respect to pseudo.  S = (degree + 1)^D, degree 1..3; csrc/spline.cu states the convention.
+    Pseudo-coordinates outside [0, 1] give indices reduced into [0, kernel_size) by a non-negative modulo."""
+    return _SplineBasis.apply(pseudo, kernel_size, is_open_spline, int(degree), wi_dtype)
+
+
+class _SplineWeighting(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x: Tensor, weight: Tensor, basis: Tensor, wi: Tensor):
+        ctx.save_for_backward(x, weight, basis, wi)
+        return ops.spline_weighting(x, weight, basis, wi)
+
+    @staticmethod
+    def backward(ctx, grad_out: Tensor):
+        x, weight, basis, wi = ctx.saved_tensors
+        need_x, need_w, need_b = ctx.needs_input_grad[:3]
+        gx, gb, gw = ops.spline_weighting_backward(grad_out, x, weight, basis, wi, need_x, need_b, need_w)
+        return gx, (gw.to(weight.dtype) if need_w else None), gb, None
+
+
+def spline_weighting(x: Tensor, weight: Tensor, basis: Tensor, weight_index: Tensor) -> Tensor:
+    """out[e] = sum_s basis[e, s] x[e] @ weight[weight_index[e, s]]: pyg_lib.ops.spline_weighting on CUDA float32 /
+    bfloat16, differentiable with respect to x, weight and basis.  This is the unfused path (what SplineConv's
+    `message` calls); `spline_conv_aggregate` fuses it with the aggregation."""
+    return _SplineWeighting.apply(x, weight, basis, weight_index)
+
+
+SPLINE_BLOCK_BYTES = 1 << 29      # fp32 bytes of P = [rows, K F_in] held at once by spline_conv_aggregate
+
+
+class _SplineConvAggregate(torch.autograd.Function):
+    """out = P W.view(K F_in, F_out) by destination-row blocks, P_i = REDUCE_e sum_s b_es x_j at kernel wi_es
+    (csrc/spline.cu).  Saves x, weight, basis and wi only: the backward recomputes each block's P for dW = sum_b P_b^T G_b,
+    forms dP_b = G_b W^T for the destination sweep (grad_basis and q per edge), and grad_x is one segment sum of q over
+    the transposed CSR.  Each step runs only when one of its outputs is needed.  P and the GEMMs are fp32; the output
+    has x's dtype."""
+
+    @staticmethod
+    def forward(ctx, x: Tensor, basis: Tensor, weight: Tensor, wi: Tensor, graph: CSRGraph, reduce: str):
+        K, Fi, Fo = weight.shape
+        w = weight.detach().float().reshape(K * Fi, Fo).contiguous()
+        out = torch.zeros(graph.num_dst, Fo, dtype=torch.float32, device=x.device)
+        for r0, r1 in _spline_blocks(graph.num_dst, K * Fi):
+            p = ops.spline_csr(graph.rowptr, graph.col, graph.perm, x, basis, wi, K, r0, r1, reduce, graph.plan)
+            out[r0:r1] = dense._mm(p, w)
+        ctx.graph, ctx.reduce = graph, reduce
+        ctx.save_for_backward(x, basis, weight, wi)
+        return out.to(x.dtype)
+
+    @staticmethod
+    def backward(ctx, grad_out: Tensor):
+        x, basis, weight, wi = ctx.saved_tensors
+        graph, reduce = ctx.graph, ctx.reduce
+        need_x, need_b, need_w = ctx.needs_input_grad[:3]
+        K, Fi, Fo = weight.shape
+        w = weight.detach().float().reshape(K * Fi, Fo).contiguous()
+        g = grad_out.float().contiguous()
+        E, S = basis.shape
+        gb = torch.empty(E, S, dtype=x.dtype, device=x.device) if need_b else None
+        q = torch.empty(E, Fi, dtype=x.dtype, device=x.device) if need_x else None
+        gw = None
+        for r0, r1 in _spline_blocks(graph.num_dst, K * Fi):
+            g_b = g[r0:r1]
+            if need_w:
+                p = ops.spline_csr(graph.rowptr, graph.col, graph.perm, x, basis, wi, K, r0, r1, reduce, graph.plan)
+                part = dense._mm_tn(p, g_b)
+                gw = part if gw is None else gw + part
+                del p
+            if need_x or need_b:
+                dp = dense._mm_nt(g_b, w).contiguous()
+                ops.spline_backward_dst(graph.rowptr, graph.col, graph.perm, x, basis, wi, K, dp, r0, r1, gb, q, reduce,
+                                        graph.plan)
+        if need_w and gw is None:
+            gw = torch.zeros_like(w)
+        gx = None
+        if need_x:
+            graph.build_transpose()
+            # grad_x[j] = the sum of q over j's out-edges: perm_t is the caller's edge id of each transposed slot
+            gx = ops.spmm_csr(graph.rowptr_t, graph.perm_t, None, q, graph.num_src, "sum", graph.plan_t)
+        gw = gw.reshape(K, Fi, Fo).to(weight.dtype) if need_w else None
+        return gx, gb, gw, None, None, None
+
+
+def _spline_blocks(n_dst: int, width: int):
+    """Destination row ranges [r0, r1) whose P fits SPLINE_BLOCK_BYTES (at least one row each)."""
+    rows = max(1, SPLINE_BLOCK_BYTES // (4 * width))
+    return [(r0, min(r0 + rows, n_dst)) for r0 in range(0, n_dst, rows)]
+
+
+def spline_conv_aggregate(graph: CSRGraph, x_src: Tensor, basis: Tensor, wi: Tensor, weight: Tensor,
+                          reduce: str = "sum") -> Tensor:
+    """out[i] = REDUCE_{e = (j -> i)} sum_s basis[e, s] x[j] @ weight[wi[e, s]] for reduce in {sum, mean}: SplineConv's
+    message and aggregation (spline_conv.py:150-153) as one CSR sweep into P [N, K F_in] and one GEMM with
+    weight.view(K F_in, F_out), without the [E, F_out] messages.  basis [E, S] of x's dtype and wi [E, S] (int32, or
+    int64 converted once) in the caller's edge order, as `spline_basis` returns them; weight [K, F_in, F_out].  x_src,
+    basis and weight may require grad.  Destination rows are processed in blocks whose fp32 P stays under
+    SPLINE_BLOCK_BYTES; a block never splits a row."""
+    if reduce not in ("sum", "add", "mean"):
+        raise ValueError(f"spline_conv_aggregate reduces by sum or mean, got '{reduce}'")
+    if x_src.dim() != 2 or x_src.size(0) != graph.num_src:
+        raise ValueError(f"x_src must be a [{graph.num_src}, F_in] tensor, got {tuple(x_src.shape)}")
+    if basis.dim() != 2 or basis.size(0) != graph.num_edges or basis.dtype != x_src.dtype \
+            or tuple(wi.shape) != tuple(basis.shape):
+        raise ValueError(f"basis and wi must be [{graph.num_edges}, S] tensors, basis of x's dtype, got "
+                         f"{tuple(basis.shape)} {basis.dtype} and {tuple(wi.shape)}")
+    if weight.dim() != 3 or weight.size(1) != x_src.size(1) or weight.dtype != x_src.dtype:
+        raise ValueError(f"weight must be a [K, {x_src.size(1)}, F_out] tensor of x's dtype, got {tuple(weight.shape)} "
+                         f"{weight.dtype}")
+    K, Fi = weight.size(0), weight.size(1)
+    if not ops.spline_supported(K, Fi, basis.size(1), x_src.dtype):
+        raise ValueError(f"spline_conv_aggregate does not take K = {K}, F_in = {Fi}, S = {basis.size(1)} in "
+                         f"{x_src.dtype}")
+    return _SplineConvAggregate.apply(x_src.contiguous(), basis.contiguous(), weight,
+                                      wi.to(torch.int32).contiguous(), graph, "mean" if reduce == "mean" else "sum")
+
+
 def _param_aggr_operands(graph, x: Optional[Tensor], a: Optional[Tensor], w, name: str, what: str):
     """The operands of softmax_aggregate and power_mean_aggregate: (x, a, w, where, want_saved).  `where` holds the
     sweep's (rowptr, col, perm, plan, n_edges, graph); w (t or p) becomes None for a Python 1 (the reference then

@@ -2,4 +2,4 @@ from .aggr import (Aggregation, FusedAggregation, MaxAggregation, MeanAggregatio
                    MinAggregation, MultiAggregation, PowerMeanAggregation, QuantileAggregation, SoftmaxAggregation,
                    StdAggregation, SumAggregation, VarAggregation, aggregation_resolver)
 from .conv import (CGConv, FastRGCNConv, GATConv, GATv2Conv, GCNConv, GENConv, GINConv, GINEConv, GraphConv, HeteroLinear,  # noqa: F401
-                   NNConv, PNAConv, ResGatedGraphConv, RGCNConv, SAGEConv, TransformerConv)
+                   NNConv, PNAConv, ResGatedGraphConv, RGCNConv, SAGEConv, SplineConv, TransformerConv)

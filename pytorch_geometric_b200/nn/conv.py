@@ -15,6 +15,7 @@ Two layers of code:
       ResGatedGraphConv nn/conv/res_gated_graph_conv.py:13-148  lin_key/lin_query/lin_value.weight/bias, lin_skip.weight, bias
       CGConv          nn/conv/cg_conv.py:12-101          lin_f.weight/bias, lin_s.weight/bias, bn.* (batch_norm)
       NNConv          nn/conv/nn_conv.py:13-126          nn.*, lin.weight (root_weight), bias
+      SplineConv      nn/conv/spline_conv.py:21-172      weight [K,in,out], bias, kernel_size/is_open_spline (buffers), lin.weight
       GENConv         nn/conv/gen_conv.py:45-243         aggr_module.t/p, lin_src/lin_edge/lin_dst.weight, mlp.*, msg_norm.scale
       PNAConv         nn/conv/pna_conv.py:20-209         aggr_module.avg_deg_lin/log, edge_encoder.*, pre_nns.t.0.*, post_nns.*, lin.*
       RGCNConv        nn/conv/rgcn_conv.py:40-300        weight [R,in,out] (or bases/blocks + comp), root, bias
@@ -714,6 +715,74 @@ class NNConv(torch.nn.Module):
 
     def __repr__(self) -> str:
         return f"{self.__class__.__name__}({self.in_channels}, {self.out_channels}, aggr={self.aggr}, nn={self.nn})"
+
+
+def _repeat(v, n: int) -> list:
+    """torch_geometric.utils.repeat: a scalar n times, a shorter list padded with its last element."""
+    if not isinstance(v, (list, tuple)):
+        return [v] * n
+    v = list(v)
+    return v + [v[-1]] * (n - len(v)) if len(v) < n else v[:n]
+
+
+def spline_conv_forward(x_src: Tensor, graph: CSRGraph, pseudo: Tensor, kernel_size: Tensor, is_open_spline: Tensor,
+                        degree: int, weight: Tensor, reduce: str) -> Tensor:
+    """SplineConv's message and aggregation (spline_conv.py:128-153): the CUDA basis of the pseudo-coordinates in int32
+    weight indices, then one CSR sweep into P and one GEMM (`Fn.spline_conv_aggregate`)."""
+    basis, wi = Fn.spline_basis(pseudo, kernel_size, is_open_spline, degree, torch.int32)
+    return Fn.spline_conv_aggregate(graph, x_src, basis, wi, weight, reduce)
+
+
+class SplineConv(torch.nn.Module):
+    """x_i Theta + AGGR_j x_j h_Theta(e_ij) + bias (spline_conv.py:21-172) with AGGR = mean (default) or sum and h the
+    B-spline kernel over the pseudo-coordinates `edge_attr` [E, dim].  The basis runs on CUDA and the message runs with
+    its aggregation as one sweep into P plus one GEMM (`Fn.spline_conv_aggregate`).  Other aggregations, lazy input
+    sizes and shapes the sweeps do not take raise ValueError."""
+
+    def __init__(self, in_channels, out_channels: int, dim: int, kernel_size, is_open_spline=True, degree: int = 1,
+                 aggr: str = "mean", root_weight: bool = True, bias: bool = True, **kwargs):
+        super().__init__()
+        if aggr not in ("add", "sum", "mean"):
+            raise ValueError(f"aggr='{aggr}' is not on the fused path (add, sum or mean)")
+        ch = (in_channels, in_channels) if isinstance(in_channels, int) else tuple(in_channels)
+        if ch[0] <= 0 or ch[1] <= 0:
+            raise ValueError("SplineConv needs its input sizes at construction (no lazy -1)")
+        self.in_channels, self.out_channels, self.dim = in_channels, out_channels, dim
+        self.degree, self.root_weight, self.aggr = degree, root_weight, aggr
+        self.flow = kwargs.get("flow", "source_to_target")
+        self.register_buffer("kernel_size", torch.tensor(_repeat(kernel_size, dim), dtype=torch.long))
+        self.register_buffer("is_open_spline", torch.tensor(_repeat(is_open_spline, dim), dtype=torch.uint8))
+        self.K = int(self.kernel_size.prod().item())
+        S = ops.spline_slots(dim, degree)
+        if not ops.spline_supported(self.K, ch[0], S, torch.float32):
+            raise ValueError(f"K = {self.K} kernels x F_in = {ch[0]} channels with {S} basis slots is outside what the "
+                             "fused SplineConv takes")
+        self.weight = torch.nn.Parameter(torch.empty(self.K, ch[0], out_channels))
+        if root_weight:
+            self.lin = _Lin(ch[1], out_channels, bias=False)      # draws as the reference's Linear(.., 'uniform') does
+        self.bias = torch.nn.Parameter(torch.zeros(out_channels)) if bias else None
+        with torch.no_grad():                                     # spline_conv.py:118-125, in the reference's order
+            bound = 1.0 / math.sqrt(self.K * ch[0])
+            self.weight.uniform_(-bound, bound)
+            if root_weight:
+                bound = 1.0 / math.sqrt(ch[1])
+                self.lin.weight.uniform_(-bound, bound)
+
+    def forward(self, x, edge_index: Adj, edge_attr: Tensor, size=None) -> Tensor:
+        pair = _pair(x)
+        if torch.is_autocast_enabled(pair[0].device.type):
+            raise ValueError("SplineConv runs in the dtype of its inputs; it does not run under torch.autocast")
+        graph = _plain_graph(edge_index, pair[0].size(0), _num_dst(pair, size), self.flow)
+        out = spline_conv_forward(pair[0], graph, edge_attr, self.kernel_size, self.is_open_spline, self.degree,
+                                  self.weight, "mean" if self.aggr == "mean" else "sum")
+        if pair[1] is not None and self.root_weight:                                  # spline_conv.py:140-145
+            out = out + self.lin(pair[1])
+        if self.bias is not None:
+            out = out + self.bias
+        return out
+
+    def __repr__(self) -> str:
+        return f"{self.__class__.__name__}({self.in_channels}, {self.out_channels}, dim={self.dim})"
 
 
 def pna_uv_c(x: Tensor, edge_attr: Optional[Tensor], pre_weights, pre_biases, enc_w: Optional[Tensor],

@@ -659,6 +659,173 @@ def nn_conv_backward_dst(rowptr: Tensor, col: Tensor, perm: Optional[Tensor], x:
            REDUCE[reduce], *_plan_rows(plan), it, _vdt(x), _stream())
 
 
+def spline_supported(k: int, f_in: int, s: int, dtype: torch.dtype) -> bool:
+    """Whether the SplineConv sweeps take K kernel weights, F_in source channels and S basis slots in this dtype."""
+    if dtype not in (torch.float32, torch.bfloat16):
+        return False
+    return bool(lib().b200mp_spline_supported(int(k), int(f_in), int(s), F32 if dtype == torch.float32 else BF16))
+
+
+def _spline_values(*ts: Optional[Tensor]) -> None:
+    for t in ts:
+        if t is not None and (not t.is_cuda or t.dtype not in (torch.float32, torch.bfloat16)):
+            raise RuntimeError("pytorch_geometric_b200 computes the spline ops on CUDA float32 / bfloat16 tensors only "
+                               f"(it has no CPU, float16 or float64 path); got a {t.dtype} tensor on {t.device}")
+
+
+def spline_slots(dim: int, degree: int) -> int:
+    """S = (degree + 1)^dim basis slots per edge; ValueError outside degree 1..3 and the slots the kernels take."""
+    if degree not in (1, 2, 3) or dim < 1:
+        raise ValueError(f"the spline ops take degree 1, 2 or 3 and dim >= 1, got degree {degree}, dim {dim}")
+    s = (degree + 1) ** dim
+    if not lib().b200mp_spline_supported(1, 1, min(s, 1 << 20), F32):
+        raise ValueError(f"(degree + 1)^dim = {s} basis slots per edge is more than the spline kernels take")
+    return s
+
+
+def _spline_knots(pseudo: Tensor, kernel_size: Tensor, is_open_spline: Tensor) -> Tuple[Tensor, Tensor]:
+    if pseudo.dim() != 2 or kernel_size.numel() != pseudo.size(1) or is_open_spline.numel() != pseudo.size(1):
+        raise ValueError(f"pseudo must be [E, D] with D kernel sizes and open flags, got {tuple(pseudo.shape)}, "
+                         f"{kernel_size.numel()} and {is_open_spline.numel()}")
+    return (kernel_size.to(device=pseudo.device, dtype=torch.int64).contiguous(),
+            is_open_spline.to(device=pseudo.device, dtype=torch.uint8).contiguous())
+
+
+def spline_basis(pseudo: Tensor, kernel_size: Tensor, is_open_spline: Tensor, degree: int,
+                 wi_dtype: torch.dtype = torch.int64) -> Tuple[Tensor, Tensor]:
+    """(basis [E, S] of pseudo's dtype, weight_index [E, S] of wi_dtype) of the B-spline tensor-product basis, S =
+    (degree + 1)^D (pyg_lib.ops.spline_basis; csrc/spline.cu states the convention)."""
+    _spline_values(pseudo)
+    ks, op = _spline_knots(pseudo, kernel_size, is_open_spline)
+    E, D = pseudo.shape
+    S = spline_slots(D, degree)
+    pseudo = pseudo.contiguous()
+    basis = torch.empty(E, S, dtype=pseudo.dtype, device=pseudo.device)
+    wi = torch.empty(E, S, dtype=wi_dtype, device=pseudo.device)
+    _timed("spline_basis", 1, lib().b200mp_spline_basis, _p(pseudo), _p(ks), _p(op), _p(basis), _p(wi), E, D, int(degree),
+           _vdt(pseudo), _idt(wi), _stream())
+    return basis, wi
+
+
+def spline_basis_backward(grad_basis: Tensor, pseudo: Tensor, kernel_size: Tensor, is_open_spline: Tensor,
+                          degree: int) -> Tensor:
+    """grad_pseudo [E, D] = sum_s grad_basis[e, s] d basis[e, s] / d pseudo[e, d]."""
+    _spline_values(pseudo, grad_basis)
+    ks, op = _spline_knots(pseudo, kernel_size, is_open_spline)
+    E, D = pseudo.shape
+    S = spline_slots(D, degree)
+    if tuple(grad_basis.shape) != (E, S):
+        raise ValueError(f"grad_basis must be [{E}, {S}], got {tuple(grad_basis.shape)}")
+    pseudo = pseudo.contiguous()
+    gb = grad_basis.to(pseudo.dtype).contiguous()
+    gp = torch.empty_like(pseudo)
+    _timed("spline_basis_backward", 1, lib().b200mp_spline_basis_backward, _p(gb), _p(pseudo), _p(ks), _p(op), _p(gp),
+           E, D, int(degree), _vdt(pseudo), _stream())
+    return gp
+
+
+def _spline_weighting_operands(x: Tensor, weight: Tensor, basis: Tensor, wi: Tensor):
+    _spline_values(x, weight, basis)
+    _cuda(wi)
+    if x.dim() != 2 or weight.dim() != 3 or weight.size(1) != x.size(1) or basis.dim() != 2 \
+            or basis.size(0) != x.size(0) or tuple(wi.shape) != tuple(basis.shape):
+        raise ValueError(f"spline_weighting takes x [E, F_in], weight [K, F_in, F_out], basis and weight_index [E, S]; "
+                         f"got {tuple(x.shape)}, {tuple(weight.shape)}, {tuple(basis.shape)}, {tuple(wi.shape)}")
+    if len({x.dtype, weight.dtype, basis.dtype}) != 1:
+        raise TypeError(f"x, weight and basis must share a dtype, got {x.dtype}, {weight.dtype}, {basis.dtype}")
+    if not lib().b200mp_spline_supported(1, 1, basis.size(1), F32):
+        raise ValueError(f"{basis.size(1)} basis slots per edge is more than the spline kernels take")
+    return x.contiguous(), weight.contiguous(), basis.contiguous(), wi.contiguous()
+
+
+def spline_weighting(x: Tensor, weight: Tensor, basis: Tensor, wi: Tensor) -> Tensor:
+    """out[e] = sum_s basis[e, s] x[e] @ weight[wi[e, s]] (pyg_lib.ops.spline_weighting), unfused: one thread per output
+    element, S F_in F_out FMAs per edge."""
+    x, weight, basis, wi = _spline_weighting_operands(x, weight, basis, wi)
+    (E, Fi), (K, _, Fo), S = x.shape, weight.shape, basis.size(1)
+    out = torch.empty(E, Fo, dtype=x.dtype, device=x.device)
+    _timed("spline_weighting", 1, lib().b200mp_spline_weighting, _p(x), _p(weight), _p(basis), _p(wi), _p(out), E, Fi, Fo,
+           K, S, _idt(wi), _vdt(x), _stream())
+    return out
+
+
+def spline_weighting_backward(grad_out: Tensor, x: Tensor, weight: Tensor, basis: Tensor, wi: Tensor, need_x: bool,
+                              need_basis: bool, need_weight: bool):
+    """(grad_x, grad_basis, grad_weight) of spline_weighting, each None unless asked for; grad_weight is fp32 and sums
+    each kernel's slots in the order of a stable sort of weight_index (one kernel per weight index, no atomics)."""
+    x, weight, basis, wi = _spline_weighting_operands(x, weight, basis, wi)
+    (E, Fi), (K, _, Fo), S = x.shape, weight.shape, basis.size(1)
+    _spline_values(grad_out)
+    g = grad_out.to(x.dtype).contiguous()
+    gx = torch.empty_like(x) if need_x else None
+    gb = torch.empty_like(basis) if need_basis else None
+    gw = torch.empty(K, Fi, Fo, dtype=torch.float32, device=x.device) if need_weight else None
+    order = ptr = None
+    if need_weight and E > 0:
+        mn, mx, _ = index_stats(wi.reshape(-1))
+        if mn < 0 or mx >= K:
+            raise IndexError(f"weight_index holds {mn}..{mx}, outside the weight's {K} kernels")
+        _, order, ptr = sort_by_key(wi.reshape(-1), K, want_sorted=False)
+    _timed("spline_weighting_backward", int(need_x) + int(need_basis) + int(need_weight),
+           lib().b200mp_spline_weighting_backward, _p(g), _p(x), _p(weight), _p(basis), _p(wi), _p(order), _p(ptr),
+           _p(gx), _p(gb), _p(gw), E, Fi, Fo, K, S, _idt(wi), _vdt(x), _stream())
+    return gx, gb, gw
+
+
+def _spline_sweep_operands(col: Tensor, x: Tensor, basis: Tensor, wi: Tensor):
+    if x.dim() != 2 or basis.dim() != 2 or basis.size(0) != col.numel() or basis.dtype != x.dtype \
+            or tuple(wi.shape) != tuple(basis.shape) or wi.dtype != torch.int32:
+        raise ValueError(f"x must be [n_src, F_in], basis [{col.numel()}, S] of x's dtype and weight_index int32 of "
+                         f"basis's shape, got {tuple(x.shape)} {x.dtype}, {tuple(basis.shape)} {basis.dtype}, "
+                         f"{tuple(wi.shape)} {wi.dtype}")
+    return x.contiguous(), basis.contiguous(), wi.contiguous(), x.size(1), basis.size(1)
+
+
+def spline_csr(rowptr: Tensor, col: Tensor, perm: Optional[Tensor], x: Tensor, basis: Tensor, wi: Tensor, k: int,
+               row_begin: int, row_end: int, reduce: str = "sum", plan: Optional[LongRowPlan] = None) -> Tensor:
+    """P [row_end - row_begin, K F_in] fp32 with P[i, k F_in + a] = REDUCE_{e in row i} sum_{s: wi[e', s] = k}
+    basis[e', s] x[col[e], a], e' = perm[e], for sum / mean: SplineConv's message before its weight (out = P W.view(K F_in,
+    F_out)).  basis [E, S] and wi [E, S] int32 in the caller's edge order; perm: CSR slot -> caller's edge id, None for
+    an adopted CSR."""
+    _cuda(rowptr, col, perm, x, basis, wi)
+    if reduce not in ("sum", "add", "mean"):
+        raise ValueError(f"spline_csr reduces by sum or mean, not '{reduce}'")
+    x, basis, wi, Fi, S = _spline_sweep_operands(col, x, basis, wi)
+    it = _same_idx(rowptr, col, perm)
+    width = int(k) * Fi
+    p = torch.empty(row_end - row_begin, width, dtype=torch.float32, device=x.device)
+    # the hub chunks' partials, n_chunks * K F_in fp32, live for this call only (as nn_conv_csr's)
+    part = None if plan is None or not plan.n_long else \
+        torch.empty(plan.n_chunks * width, dtype=torch.float32, device=x.device)
+    pargs = (*_plan_rows(plan), _p(part))
+    _timed("spline_csr", 2 if pargs[2] else 1, lib().b200mp_spline_csr, _p(rowptr), _p(col), _p(perm), _p(x), _p(basis),
+           _p(wi), _p(p), rowptr.numel() - 1, x.size(0), col.numel(), int(k), Fi, S, int(row_begin), int(row_end),
+           REDUCE[reduce], *pargs, it, _vdt(x), _stream())
+    return p
+
+
+def spline_backward_dst(rowptr: Tensor, col: Tensor, perm: Optional[Tensor], x: Tensor, basis: Tensor, wi: Tensor,
+                        k: int, grad_p: Tensor, row_begin: int, row_end: int, grad_basis: Optional[Tensor],
+                        q: Optional[Tensor], reduce: str = "sum", plan: Optional[LongRowPlan] = None) -> None:
+    """Destination sweep of the fused SplineConv's backward for rows [row_begin, row_end): writes, per edge in the
+    caller's order, grad_basis[e, s] = <grad_p[i, wi[e, s], :], x_j> into `grad_basis` ([E, S]) and q[e, :] =
+    sum_s basis[e, s] grad_p[i, wi[e, s], :] into `q` ([E, F_in]), either None to skip it.  grad_p: fp32
+    [row_end - row_begin, K F_in]."""
+    _cuda(rowptr, col, perm, x, basis, wi, grad_p, grad_basis, q)
+    x, basis, wi, Fi, S = _spline_sweep_operands(col, x, basis, wi)
+    E = col.numel()
+    if tuple(grad_p.shape) != (row_end - row_begin, int(k) * Fi) or grad_p.dtype != torch.float32 \
+            or not grad_p.is_contiguous():
+        raise ValueError(f"grad_p must be a contiguous fp32 [{row_end - row_begin}, {int(k) * Fi}] tensor")
+    for name, t, w in (("grad_basis", grad_basis, S), ("q", q, Fi)):
+        if t is not None and (tuple(t.shape) != (E, w) or t.dtype != x.dtype or not t.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous [{E}, {w}] tensor of x's dtype")
+    it = _same_idx(rowptr, col, perm)
+    _timed("spline_backward_dst", 1, lib().b200mp_spline_backward_dst, _p(rowptr), _p(col), _p(perm), _p(x), _p(basis),
+           _p(wi), _p(grad_p), _p(grad_basis), _p(q), rowptr.numel() - 1, x.size(0), E, int(k), Fi, S, int(row_begin),
+           int(row_end), REDUCE[reduce], *_plan_rows(plan), it, _vdt(x), _stream())
+
+
 SOFTMAX_MESSAGES = {"identity": 0, "relu_eps": 1}
 
 

@@ -118,10 +118,21 @@ def install(layers: bool = False, extensions: bool = True, flip_flags: bool = Fa
                     _set(mod, attr, shim)
                     n += 1
         counts["extension_modules"] = n
+        # SplineConv imports spline_basis / spline_weighting by name and leaves them None without pyg-lib
+        # (nn/conv/spline_conv.py:15-18); its constructor raises ImportError until they are bound
+        import torch_geometric.nn.conv.spline_conv as tg_spline
+        k = 0
+        for name in ("spline_basis", "spline_weighting"):
+            if getattr(tg_spline, name, None) is None:
+                _set(tg_spline, name, getattr(pl.ops, name))
+                k += 1
+        counts["spline_ops"] = k
         if flip_flags:
             for flag in ("WITH_TORCH_SCATTER", "WITH_SOFTMAX", "WITH_INDEX_SORT", "WITH_SEGMM", "WITH_GMM"):
                 _set(tg_typing, flag, True)
             counts["flags"] = 5
+            _set(tg_typing, "WITH_SPLINE", True)
+            counts["spline_flag"] = 1
 
     if layers:
         import torch_geometric.nn as tgnn

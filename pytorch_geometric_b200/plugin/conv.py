@@ -37,7 +37,8 @@ from ._util import plain
 # Inspector caches class sources by `cls.__name__` (torch_geometric/inspector.py:323-334), so a subclass that reused
 # its parent's name would hide the parent's `# propagate_type:` annotation and get a `propagate` without arguments.
 LAYERS = {n: "B200" + n for n in ("GCNConv", "SAGEConv", "GraphConv", "GINConv", "GATConv", "GATv2Conv", "TransformerConv",
-                                  "RGCNConv", "FastRGCNConv", "PNAConv", "CGConv", "GENConv", "NNConv")}
+                                  "RGCNConv", "FastRGCNConv", "PNAConv", "CGConv", "GENConv", "NNConv",
+                                  "SplineConv")}
 LAYERS["ECConv"] = "B200NNConv"                 # the reference's alias of NNConv (nn/conv/__init__.py)
 
 
@@ -446,6 +447,47 @@ class B200NNConv(tgnn.NNConv):
                 reduce = "mean" if type(self.aggr_module) is tgnn.aggr.MeanAggregation else "sum"
                 out = Fn.nn_conv_aggregate(g, xs[0], h, w_prime, reduce)
                 if xs[1] is not None and self.root_weight:                             # nn_conv.py:110-115
+                    out = out + self.lin(xs[1])
+                if self.bias is not None:
+                    out = out + self.bias
+                return out
+        return super().forward(x, edge_index, edge_attr, size)
+
+
+def _spline_fusable(self, xs, edge_index, edge_attr) -> bool:
+    """Whether the fused SplineConv path covers the call: sum / mean aggregation, a 2-D edge_attr with `dim` columns, a
+    [2, E] tensor or EdgeIndex adjacency, CUDA float32 / bfloat16 tensors and parameters of one dtype outside
+    torch.autocast, no hooks, explain, decomposed layers or compiling, and a shape the sweeps take."""
+    if type(self.aggr_module) not in (tgnn.aggr.SumAggregation, tgnn.aggr.MeanAggregation):
+        return False
+    if xs[0] is None or xs[0].dim() != 2 or torch.is_autocast_enabled(xs[0].device.type):
+        return False
+    if not isinstance(edge_attr, Tensor) or edge_attr.dim() != 2 or edge_attr.size(1) != self.dim:
+        return False
+    if not (isinstance(edge_index, Tensor) and edge_index.layout == torch.strided and edge_index.dim() == 2
+            and edge_index.size(0) == 2 and not edge_index.is_floating_point()):
+        return False
+    if isinstance(self.weight, torch.nn.parameter.UninitializedParameter) or self.weight.size(1) != xs[0].size(1):
+        return False
+    ts = [t for t in (xs[0], xs[1], edge_attr) if t is not None]
+    if not _fast(self, *ts) or len({t.dtype for t in ts} | {p.dtype for p in self.parameters()}) != 1:
+        return False
+    if self.degree not in (1, 2, 3):
+        return False
+    s = (self.degree + 1) ** self.dim
+    return ops.spline_supported(self.weight.size(0), self.weight.size(1), s, xs[0].dtype)
+
+
+class B200SplineConv(tgnn.SplineConv):
+    def forward(self, x, edge_index, edge_attr=None, size=None) -> Tensor:
+        xs = _pair(x)
+        if _spline_fusable(self, xs, edge_index, edge_attr):
+            g = _graph(edge_index, xs[0].size(0), _ndst(xs, size), self.flow)
+            if g is not None:
+                reduce = "mean" if type(self.aggr_module) is tgnn.aggr.MeanAggregation else "sum"
+                out = C.spline_conv_forward(xs[0], g, edge_attr, self.kernel_size, self.is_open_spline, self.degree,
+                                            self.weight, reduce)
+                if xs[1] is not None and self.root_weight:                             # spline_conv.py:140-145
                     out = out + self.lin(xs[1])
                 if self.bias is not None:
                     out = out + self.bias

@@ -11,8 +11,11 @@ engine: flipping `torch_geometric.typing.WITH_*` to True with these modules boun
   pyg_lib.ops.softmax_csr(src, ptr, dim)                                           utils/_softmax.py:58
   pyg_lib.ops.index_sort(inputs, max_value) -> (values, perm)                      utils/_index_sort.py:32
   pyg_lib.ops.segment_matmul(inputs, ptr, other) / grouped_matmul(inputs, others, biases)   nn/dense/linear.py:255,304-330
+  pyg_lib.ops.spline_basis(pseudo, kernel_size, is_open_spline, degree) -> (basis, weight_index)  nn/conv/spline_conv.py:151
+  pyg_lib.ops.spline_weighting(x, weight, basis, weight_index)                     nn/conv/spline_conv.py:153
 
-CUDA fp32 / bf16 operands run in the engine.  CPU operands fall through to the reference's own ATen branch (the
+CUDA fp32 / bf16 operands run in the engine.  The spline ops have no reference fall-back (the reference has no ATen
+branch for them), so CPU, float16 and float64 operands raise RuntimeError.  Other CPU operands fall through to the reference's own ATen branch (the
 shim calls the reference function with the extension flag switched off for the duration of the call) -- the engine
 itself never computes on the CPU.  torch.ops.torch_sparse.* are `torch.library` operators with a CUDA implementation,
 a Meta (shape) implementation so tracing stays legal, and autograd formulas that use the transposed structure the
@@ -282,6 +285,14 @@ def _pl_grouped_matmul(inputs: List[Tensor], others: List[Tensor], biases: Optio
     return dense.grouped_matmul(inputs, others, biases)
 
 
+def _pl_spline_basis(pseudo: Tensor, kernel_size: Tensor, is_open_spline: Tensor, degree: int) -> Tuple[Tensor, Tensor]:
+    return Fn.spline_basis(pseudo, kernel_size, is_open_spline, degree)
+
+
+def _pl_spline_weighting(x: Tensor, weight: Tensor, basis: Tensor, weight_index: Tensor) -> Tensor:
+    return Fn.spline_weighting(x, weight, basis, weight_index)
+
+
 def pyg_lib_module() -> types.ModuleType:
     m = types.ModuleType("pyg_lib")
     m.__doc__ = "pytorch_geometric_b200 shim of the pyg_lib.ops operators on the aggregation path"
@@ -290,5 +301,7 @@ def pyg_lib_module() -> types.ModuleType:
     m.ops.index_sort = _pl_index_sort
     m.ops.segment_matmul = _pl_segment_matmul
     m.ops.grouped_matmul = _pl_grouped_matmul
+    m.ops.spline_basis = _pl_spline_basis
+    m.ops.spline_weighting = _pl_spline_weighting
     m.__version__ = "b200mp-shim"
     return m

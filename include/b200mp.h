@@ -565,6 +565,54 @@ int b200mp_spline_backward_dst(const void* rowptr, const void* col, const void* 
                                const int64_t* plan_chunk_ptr, int64_t plan_n_long, int64_t plan_n_chunks,
                                int64_t plan_chunk, int idx_dtype, int val_dtype, void* stream);
 
+/* ------------------------------------------------------------------ point clouds (k-NN, radius, fps, nearest)
+ * Replace pyg_lib.ops.knn / radius / fps / nearest (torch.ops.pyg.*, nn/pool/__init__.py:85,140,199,265,331,375).
+ * Points: x [n_x, f], y [n_y, f] row-major (val_dtype, fp32 or bf16, widened exactly to fp32); n_x < 2^31.  Examples:
+ * ptr_x [n_ptr_x] / ptr_y [n_ptr_y] (ptr_dtype, one dtype for both) give example b the range ptr[b]:ptr[b+1]; a NULL
+ * ptr is one example covering every point, and examples missing at the end of the shorter ptr are empty.
+ * Distances: d = sum_f (x_f - y_f)^2, or 1 - dot / (sqrt(|x|^2) sqrt(|y|^2)) under cosine, every sum in feature order with
+ * explicitly rounded fp32 operations (no FMA contraction); a candidate is selected only when d compares below something
+ * with a strict <, so NaN and infinite distances are never selected.  Outputs are int64; offsets [n + 1] are written as
+ * exclusive offsets of the per-query lengths (offsets[n] is the total, the caller's one device-to-host read). */
+/* k nearest x points of each query's example, 1 <= k <= 128 (else B200MP_ERR_UNSUPPORTED): slab [2, n_y k] gets, for
+ * query i, row i in slab[0, i k + c] and the c-th neighbour in slab[1, i k + c] (distance ascending, ties by ascending x
+ * index; -1 past the query's length), and offsets [n_y + 1] the offsets of the lengths.  When offsets[n_y] == n_y k the
+ * slab is the [2, nnz] result; otherwise b200mp_knn_compact packs it. */
+int b200mp_knn(const void* x, const void* y, const void* ptr_x, const void* ptr_y, int64_t n_x, int64_t n_y, int64_t f,
+               int64_t n_ptr_x, int64_t n_ptr_y, int64_t k, int cosine, int64_t* slab, int64_t* offsets, int val_dtype,
+               int ptr_dtype, void* stream);
+/* out [2, nnz] = the slab's first offsets[i+1] - offsets[i] entries of each query, queries ascending. */
+int b200mp_knn_compact(const int64_t* slab, const int64_t* offsets, int64_t n_y, int64_t k, int64_t* out, int64_t nnz,
+                       void* stream);
+/* Radius, pass 1: offsets [n_y + 1] of the number of x points of each query's example with d < r2 (squared distance;
+ * r2 is the caller's fp64 r * r rounded once to fp32), capped at max_num_neighbors, skipping x index == y index when
+ * ignore_same_index is set. */
+int b200mp_radius_count(const void* x, const void* y, const void* ptr_x, const void* ptr_y, int64_t n_x, int64_t n_y,
+                        int64_t f, int64_t n_ptr_x, int64_t n_ptr_y, float r2, int64_t max_num_neighbors,
+                        int ignore_same_index, int64_t* offsets, int val_dtype, int ptr_dtype, void* stream);
+/* Radius, pass 2: out [2, nnz] (nnz = offsets[n_y]) gets (y index, x index) pairs, queries ascending and each query's
+ * first max_num_neighbors x points in ascending index order. */
+int b200mp_radius_fill(const void* x, const void* y, const void* ptr_x, const void* ptr_y, int64_t n_x, int64_t n_y,
+                       int64_t f, int64_t n_ptr_x, int64_t n_ptr_y, float r2, int64_t max_num_neighbors,
+                       int ignore_same_index, const int64_t* offsets, int64_t* out, int64_t nnz, int val_dtype,
+                       int ptr_dtype, void* stream);
+/* For each x point, the nearest y point of its example (torch-cluster's cluster vector): the k-NN sweep with k = 1 and
+ * the roles swapped.  slab [2, n_x] gets (x index, y index or -1), offsets [n_x + 1] the offsets of the lengths (0 or 1):
+ * offsets[n_x] < n_x means some x point found no y point. */
+int b200mp_nearest(const void* x, const void* y, const void* ptr_x, const void* ptr_y, int64_t n_x, int64_t n_y,
+                   int64_t f, int64_t n_ptr_x, int64_t n_ptr_y, int64_t* slab, int64_t* offsets, int val_dtype,
+                   int ptr_dtype, void* stream);
+/* Farthest-point sampling, pass 1: offsets [B + 1] of ceil(n_b ratio) (fp64) samples per example, 0 < ratio <= 1;
+ * B = n_ptr - 1, or 1 when ptr is NULL. */
+int b200mp_fps_count(const void* ptr, int64_t n_ptr, int64_t n, double ratio, int64_t* offsets, int ptr_dtype,
+                     void* stream);
+/* Pass 2: out [offsets[B]] gets each example's samples (global indices) in selection order, examples concatenated.  The
+ * start is the example's first point, or point floor(rnd[b] n_b) when rnd [B] (uniform in [0, 1), fp32) is given;
+ * each step takes the argmax of the running min squared distance, ties to the lowest index.  dist_ws [n] fp32 is the
+ * min-distance of examples too large for shared memory. */
+int b200mp_fps(const void* src, const void* ptr, int64_t n, int64_t f, int64_t n_ptr, const float* rnd,
+               const int64_t* offsets, float* dist_ws, int64_t* out, int val_dtype, int ptr_dtype, void* stream);
+
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)
  * out[index[e], :] (+)= src[e, :] for an UNSORTED index.  Replaces utils/_scatter.py:14-138
  * (aten::scatter_add_ / scatter_reduce_, torch_scatter.scatter).  fp32 only.  `count` is a

@@ -16,6 +16,7 @@ _INT = ctypes.c_int
 _P = ctypes.c_void_p
 _F = ctypes.c_float
 _U64 = ctypes.c_uint64
+_D = ctypes.c_double
 
 # name -> (restype, argtypes); mirrors include/b200mp.h one to one
 _SIGS = {
@@ -85,6 +86,13 @@ _SIGS = {
     "b200mp_spline_weighting_backward": (_INT, [_P] * 10 + [_I64] * 5 + [_INT, _INT, _P]),
     "b200mp_spline_csr": (_INT, [_P] * 7 + [_I64] * 8 + [_INT, _P, _P, _I64, _I64, _I64, _P, _INT, _INT, _P]),
     "b200mp_spline_backward_dst": (_INT, [_P] * 9 + [_I64] * 8 + [_INT, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
+    "b200mp_knn": (_INT, [_P] * 4 + [_I64] * 6 + [_INT, _P, _P, _INT, _INT, _P]),
+    "b200mp_knn_compact": (_INT, [_P, _P, _I64, _I64, _P, _I64, _P]),
+    "b200mp_radius_count": (_INT, [_P] * 4 + [_I64] * 5 + [_F, _I64, _INT, _P, _INT, _INT, _P]),
+    "b200mp_radius_fill": (_INT, [_P] * 4 + [_I64] * 5 + [_F, _I64, _INT, _P, _P, _I64, _INT, _INT, _P]),
+    "b200mp_nearest": (_INT, [_P] * 4 + [_I64] * 5 + [_P, _P, _INT, _INT, _P]),
+    "b200mp_fps_count": (_INT, [_P, _I64, _I64, _D, _P, _INT, _P]),
+    "b200mp_fps": (_INT, [_P, _P, _I64, _I64, _I64, _P, _P, _P, _P, _INT, _INT, _P]),
     "b200mp_scatter_coo": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
     "b200mp_split_tf32": (_INT, [_P, _P, _P, _I64, _P]),
     "b200mp_split_tf32_transposed": (_INT, [_P, _P, _P, _I64, _I64, _P]),

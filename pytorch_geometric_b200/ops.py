@@ -829,6 +829,142 @@ def spline_backward_dst(rowptr: Tensor, col: Tensor, perm: Optional[Tensor], x: 
 SOFTMAX_MESSAGES = {"identity": 0, "relu_eps": 1}
 
 
+# ------------------------------------------------------------------ point clouds (csrc/point.cu)
+KNN_MAX_K = 128
+
+
+def _point_values(*ts: Optional[Tensor]) -> None:
+    for t in ts:
+        if t is not None and (not t.is_cuda or t.dtype not in (torch.float32, torch.bfloat16)):
+            raise RuntimeError("pytorch_geometric_b200 computes the point-cloud ops on CUDA float32 / bfloat16 tensors "
+                               f"only (it has no CPU, float16 or float64 path); got a {t.dtype} tensor on {t.device}")
+
+
+def _point_rows(t: Tensor) -> Tensor:
+    """[N, F] contiguous view of a point matrix (a 1-D tensor is N points of one feature)."""
+    t = t.detach()
+    t = t.view(-1, 1) if t.dim() == 1 else t.reshape(t.size(0), -1)
+    return t.contiguous()
+
+
+def _point_ptrs(n_x: int, n_y: int, ptr_x: Optional[Tensor], ptr_y: Optional[Tensor], device):
+    ptrs = [p for p in (ptr_x, ptr_y) if p is not None]
+    _cuda(*ptrs)
+    for p in ptrs:
+        if p.device != device:
+            raise RuntimeError(f"ptr must be on the points' device {device}, got {p.device}")
+    pdt = _same_idx(*ptrs) if ptrs else I64
+    ptr_x = None if ptr_x is None else ptr_x.contiguous()
+    ptr_y = None if ptr_y is None else ptr_y.contiguous()
+    from . import _debug
+    if _debug.enabled():
+        for p, n, name in ((ptr_x, n_x, "ptr_x"), (ptr_y, n_y, "ptr_y")):
+            if p is not None and p.numel() > 0:
+                h = p.cpu()
+                if int(h[0]) < 0 or int(h[-1]) > n or bool((h[1:] < h[:-1]).any()):
+                    raise ValueError(f"{name} must be non-decreasing within [0, {n}]")
+    return ptr_x, ptr_y, pdt
+
+
+def _np(p: Optional[Tensor]) -> int:
+    return 0 if p is None else p.numel()
+
+
+def knn(x: Tensor, y: Tensor, k: int, ptr_x: Optional[Tensor] = None, ptr_y: Optional[Tensor] = None,
+        cosine: bool = False) -> Tensor:
+    """[2, nnz] int64 (y index, x index): for each y point the k nearest x points of its example, distance ascending,
+    ties by ascending x index (pyg_lib.ops.knn; csrc/point.cu states the distance contract)."""
+    _point_values(x, y)
+    k = int(k)
+    if not 1 <= k <= KNN_MAX_K:
+        raise ValueError(f"knn takes 1 <= k <= {KNN_MAX_K} neighbours, got k = {k}")
+    if x.dtype != y.dtype:
+        raise TypeError(f"x and y must share a dtype, got {x.dtype} and {y.dtype}")
+    x, y = _point_rows(x), _point_rows(y)
+    if x.size(1) != y.size(1):
+        raise ValueError(f"x and y must have the same number of features, got {x.size(1)} and {y.size(1)}")
+    ptr_x, ptr_y, pdt = _point_ptrs(x.size(0), y.size(0), ptr_x, ptr_y, x.device)
+    M = y.size(0)
+    slab = torch.empty(2, M * k, dtype=torch.int64, device=x.device)
+    offsets = torch.empty(M + 1, dtype=torch.int64, device=x.device)
+    _timed("knn", 2, lib().b200mp_knn, _p(x), _p(y), _p(ptr_x), _p(ptr_y), x.size(0), M, x.size(1), _np(ptr_x),
+           _np(ptr_y), k, int(bool(cosine)), _p(slab), _p(offsets), _vdt(x), pdt, _stream())
+    nnz = int(offsets[M])
+    if nnz == M * k:
+        return slab
+    out = torch.empty(2, nnz, dtype=torch.int64, device=x.device)
+    _timed("knn_compact", 1, lib().b200mp_knn_compact, _p(slab), _p(offsets), M, k, _p(out), nnz, _stream())
+    return out
+
+
+def radius(x: Tensor, y: Tensor, r: float, ptr_x: Optional[Tensor] = None, ptr_y: Optional[Tensor] = None,
+           max_num_neighbors: int = 32, ignore_same_index: bool = False) -> Tensor:
+    """[2, nnz] int64 (y index, x index): for each y point the first max_num_neighbors x points of its example, in
+    ascending index order, with squared distance < r^2 (r^2 formed in fp64, rounded once to fp32)."""
+    _point_values(x, y)
+    if x.dtype != y.dtype:
+        raise TypeError(f"x and y must share a dtype, got {x.dtype} and {y.dtype}")
+    x, y = _point_rows(x), _point_rows(y)
+    if x.size(1) != y.size(1):
+        raise ValueError(f"x and y must have the same number of features, got {x.size(1)} and {y.size(1)}")
+    ptr_x, ptr_y, pdt = _point_ptrs(x.size(0), y.size(0), ptr_x, ptr_y, x.device)
+    M = y.size(0)
+    r2 = float(r) * float(r)                                      # fp64; ctypes rounds it once to fp32
+    args = (_p(x), _p(y), _p(ptr_x), _p(ptr_y), x.size(0), M, x.size(1), _np(ptr_x), _np(ptr_y), r2,
+            int(max_num_neighbors), int(bool(ignore_same_index)))
+    offsets = torch.empty(M + 1, dtype=torch.int64, device=x.device)
+    _timed("radius_count", 2, lib().b200mp_radius_count, *args, _p(offsets), _vdt(x), pdt, _stream())
+    nnz = int(offsets[M])
+    out = torch.empty(2, nnz, dtype=torch.int64, device=x.device)
+    _timed("radius_fill", 1, lib().b200mp_radius_fill, *args, _p(offsets), _p(out), nnz, _vdt(x), pdt, _stream())
+    return out
+
+
+def nearest(x: Tensor, y: Tensor, ptr_x: Optional[Tensor] = None, ptr_y: Optional[Tensor] = None) -> Tensor:
+    """[N] int64: for each x point, the index of the nearest y point of its example (torch-cluster's cluster vector).
+    ValueError when an x point finds none (its example has no y points, or only NaN / infinite distances)."""
+    _point_values(x, y)
+    if x.dtype != y.dtype:
+        raise TypeError(f"x and y must share a dtype, got {x.dtype} and {y.dtype}")
+    x, y = _point_rows(x), _point_rows(y)
+    if x.size(1) != y.size(1):
+        raise ValueError(f"x and y must have the same number of features, got {x.size(1)} and {y.size(1)}")
+    ptr_x, ptr_y, pdt = _point_ptrs(x.size(0), y.size(0), ptr_x, ptr_y, x.device)
+    N = x.size(0)
+    slab = torch.empty(2, N, dtype=torch.int64, device=x.device)
+    offsets = torch.empty(N + 1, dtype=torch.int64, device=x.device)
+    _timed("nearest", 2, lib().b200mp_nearest, _p(x), _p(y), _p(ptr_x), _p(ptr_y), N, y.size(0), x.size(1),
+           _np(ptr_x), _np(ptr_y), _p(slab), _p(offsets), _vdt(x), pdt, _stream())
+    if int(offsets[N]) != N:
+        raise ValueError("nearest: some x point has no y point in its example (or only NaN / infinite distances)")
+    return slab[1]
+
+
+def fps(src: Tensor, ptr: Optional[Tensor] = None, ratio: float = 0.5, random_start: bool = True) -> Tensor:
+    """[S] int64 global indices of the farthest-point samples of each example, in selection order, examples
+    concatenated; ceil(n_b ratio) samples of example b (fp64), 0 < ratio <= 1.  random_start draws the start of each
+    example on the device from torch's CUDA generator; otherwise each example starts at its first point."""
+    _point_values(src)
+    ratio = float(ratio)
+    if not 0.0 < ratio <= 1.0:
+        raise ValueError(f"fps takes a sampling ratio in (0, 1], got {ratio}")
+    src = _point_rows(src)
+    N = src.size(0)
+    ptr, _, pdt = _point_ptrs(N, N, ptr, None, src.device)
+    B = 1 if ptr is None else max(ptr.numel() - 1, 0)
+    offsets = torch.empty(B + 1, dtype=torch.int64, device=src.device)
+    _timed("fps_count", 2, lib().b200mp_fps_count, _p(ptr), _np(ptr), N, ratio, _p(offsets), pdt, _stream())
+    total = int(offsets[B])
+    out = torch.empty(total, dtype=torch.int64, device=src.device)
+    if total == 0:
+        return out
+    rnd = torch.rand(B, device=src.device) if random_start else None
+    dist = torch.empty(N, dtype=torch.float32, device=src.device)
+    _timed("fps", 1, lib().b200mp_fps, _p(src), _p(ptr), N, src.size(1), _np(ptr), _p(rnd), _p(offsets), _p(dist),
+           _p(out), _vdt(src), pdt, _stream())
+    return out
+
+
 def _softmax_aggr_args(x: Optional[Tensor], a: Optional[Tensor], w: Optional[Tensor], message: str, n_edges: int,
                        clamp: Optional[tuple] = None):
     """Check the operands of the softmax- and power-mean-aggregation sweeps; returns (F, message code, mode of w), and

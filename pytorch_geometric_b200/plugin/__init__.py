@@ -127,12 +127,17 @@ def install(layers: bool = False, extensions: bool = True, flip_flags: bool = Fa
                 _set(tg_spline, name, getattr(pl.ops, name))
                 k += 1
         counts["spline_ops"] = k
+        # the point-cloud functions and DynamicEdgeConv / GravNetConv / XConv call torch.ops.pyg.* directly
+        counts["point_ops"] = shims.register_point_ops()
         if flip_flags:
             for flag in ("WITH_TORCH_SCATTER", "WITH_SOFTMAX", "WITH_INDEX_SORT", "WITH_SEGMM", "WITH_GMM"):
                 _set(tg_typing, flag, True)
             counts["flags"] = 5
             _set(tg_typing, "WITH_SPLINE", True)
             counts["spline_flag"] = 1
+            for flag in ("WITH_KNN", "WITH_RADIUS", "WITH_FPS", "WITH_NEAREST"):
+                _set(tg_typing, flag, True)
+            counts["point_flags"] = 4
 
     if layers:
         import torch_geometric.nn as tgnn

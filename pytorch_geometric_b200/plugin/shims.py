@@ -13,9 +13,11 @@ engine: flipping `torch_geometric.typing.WITH_*` to True with these modules boun
   pyg_lib.ops.segment_matmul(inputs, ptr, other) / grouped_matmul(inputs, others, biases)   nn/dense/linear.py:255,304-330
   pyg_lib.ops.spline_basis(pseudo, kernel_size, is_open_spline, degree) -> (basis, weight_index)  nn/conv/spline_conv.py:151
   pyg_lib.ops.spline_weighting(x, weight, basis, weight_index)                     nn/conv/spline_conv.py:153
+  torch.ops.pyg.knn / radius / fps / nearest (also pyg_lib.ops.*)                  nn/pool/__init__.py:85-375,
+                                                                                   nn/conv/{edge,gravnet,x}_conv.py
 
-CUDA fp32 / bf16 operands run in the engine.  The spline ops have no reference fall-back (the reference has no ATen
-branch for them), so CPU, float16 and float64 operands raise RuntimeError.  Other CPU operands fall through to the reference's own ATen branch (the
+CUDA fp32 / bf16 operands run in the engine.  The spline and point-cloud ops have no reference fall-back (the reference has no
+ATen branch for them), so CPU, float16 and float64 operands raise RuntimeError.  Other CPU operands fall through to the reference's own ATen branch (the
 shim calls the reference function with the extension flag switched off for the duration of the call) -- the engine
 itself never computes on the CPU.  torch.ops.torch_sparse.* are `torch.library` operators with a CUDA implementation,
 a Meta (shape) implementation so tracing stays legal, and autograd formulas that use the transposed structure the
@@ -293,6 +295,59 @@ def _pl_spline_weighting(x: Tensor, weight: Tensor, basis: Tensor, weight_index:
     return Fn.spline_weighting(x, weight, basis, weight_index)
 
 
+# ================================================================================================ torch.ops.pyg (point clouds)
+_POINT_LIB = None
+POINT_SCHEMAS = {
+    "knn": "knn(Tensor x, Tensor y, Tensor? ptr_x, Tensor? ptr_y, int k, bool cosine, int num_workers) -> Tensor",
+    "radius": "radius(Tensor x, Tensor y, Tensor? ptr_x, Tensor? ptr_y, float r, int max_num_neighbors, "
+              "int num_workers, bool ignore_same_index) -> Tensor",
+    "fps": "fps(Tensor src, Tensor ptr, float ratio, bool random_start) -> Tensor",
+    "nearest": "nearest(Tensor x, Tensor y, Tensor? ptr_x, Tensor? ptr_y) -> Tensor",
+}
+
+
+def _pyg_knn(x: Tensor, y: Tensor, ptr_x: Optional[Tensor], ptr_y: Optional[Tensor], k: int, cosine: bool = False,
+             num_workers: int = 1) -> Tensor:
+    return ops.knn(x, y, k, ptr_x, ptr_y, cosine)
+
+
+def _pyg_radius(x: Tensor, y: Tensor, ptr_x: Optional[Tensor], ptr_y: Optional[Tensor], r: float,
+                max_num_neighbors: int = 32, num_workers: int = 1, ignore_same_index: bool = False) -> Tensor:
+    return ops.radius(x, y, r, ptr_x, ptr_y, max_num_neighbors, ignore_same_index)
+
+
+def _pyg_fps(src: Tensor, ptr: Tensor, ratio: float = 0.5, random_start: bool = True) -> Tensor:
+    return ops.fps(src, ptr, ratio, random_start)
+
+
+def _pyg_nearest(x: Tensor, y: Tensor, ptr_x: Optional[Tensor] = None, ptr_y: Optional[Tensor] = None) -> Tensor:
+    return ops.nearest(x, y, ptr_x, ptr_y)
+
+
+POINT_OPS = {"knn": _pyg_knn, "radius": _pyg_radius, "fps": _pyg_fps, "nearest": _pyg_nearest}
+
+
+def register_point_ops() -> int:
+    """Defines torch.ops.pyg.{knn, radius, fps, nearest} with pyg-lib's schemas and CUDA implementations only.  Returns
+    the number of operators this call or an earlier one defined; an operator the namespace already has (the real
+    pyg-lib is installed) is left alone."""
+    global _POINT_LIB
+    if _POINT_LIB is not None:
+        return _POINT_LIB[1]
+    missing = []
+    for name in POINT_SCHEMAS:
+        try:
+            getattr(torch.ops.pyg, name)
+        except (AttributeError, RuntimeError):
+            missing.append(name)
+    lib = torch.library.Library("pyg", "FRAGMENT")
+    for name in missing:
+        lib.define(POINT_SCHEMAS[name])
+        lib.impl(name, POINT_OPS[name], "CUDA")
+    _POINT_LIB = (lib, len(missing))
+    return len(missing)
+
+
 def pyg_lib_module() -> types.ModuleType:
     m = types.ModuleType("pyg_lib")
     m.__doc__ = "pytorch_geometric_b200 shim of the pyg_lib.ops operators on the aggregation path"
@@ -303,5 +358,9 @@ def pyg_lib_module() -> types.ModuleType:
     m.ops.grouped_matmul = _pl_grouped_matmul
     m.ops.spline_basis = _pl_spline_basis
     m.ops.spline_weighting = _pl_spline_weighting
+    m.ops.knn = _pyg_knn
+    m.ops.radius = _pyg_radius
+    m.ops.fps = _pyg_fps
+    m.ops.nearest = _pyg_nearest
     m.__version__ = "b200mp-shim"
     return m

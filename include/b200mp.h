@@ -36,7 +36,7 @@ extern "C" {
 #define B200MP_VERSION "0.1.0"
 
 /* element / index dtypes */
-enum { B200MP_F32 = 0, B200MP_BF16 = 1 };
+enum { B200MP_F32 = 0, B200MP_BF16 = 1, B200MP_F64 = 2 };
 enum { B200MP_I32 = 0, B200MP_I64 = 1 };
 /* reductions (same codes as oracle/mp_oracle.c) */
 enum { B200MP_SUM = 0, B200MP_MEAN = 1, B200MP_MIN = 2, B200MP_MAX = 3, B200MP_MUL = 4 };
@@ -612,6 +612,26 @@ int b200mp_fps_count(const void* ptr, int64_t n_ptr, int64_t n, double ratio, in
  * min-distance of examples too large for shared memory. */
 int b200mp_fps(const void* src, const void* ptr, int64_t n, int64_t f, int64_t n_ptr, const float* rnd,
                const int64_t* offsets, float* dist_ws, int64_t* out, int val_dtype, int ptr_dtype, void* stream);
+
+/* ------------------------------------------------------------------ clustering for pooling (graclus, voxel grid)
+ * Greedy graph matching: replaces pyg_lib.ops.graclus_cluster (torch.ops.pyg.graclus_cluster, nn/pool/graclus.py:39).
+ * rowptr [n + 1] / col (idx_dtype) is the CSR adjacency, n < 2^31; weight (NULL = unweighted) is one value per CSR
+ * entry, fp32 / bf16 / fp64 (weight_dtype = B200MP_F32 / B200MP_BF16 / B200MP_F64), only compared after an exact
+ * widening to fp64.  cluster [n] int64 gets min(u, v) for each matched pair and u for each singleton.  The matching is
+ * a pure function of (graph, weight, seed): rounds of propose / respond / settle with node colours from
+ * splitmix64(seed, round * n + u), in one cooperative launch (B200MP_ERR_UNSUPPORTED on a device without cooperative
+ * launches), at most 256 rounds, after which unmatched nodes become singletons (csrc/cluster.cu states the rules).
+ * ws [2n + 3] int32 is scratch; ws[2n + 2] receives the number of rounds used.  n = 0 launches nothing. */
+int b200mp_graclus(const void* rowptr, const void* col, const void* weight, int64_t n, uint64_t seed, int64_t* cluster,
+                   int32_t* ws, int idx_dtype, int weight_dtype, void* stream);
+/* Regular-grid clustering: replaces pyg_lib.ops.grid_cluster (torch.ops.pyg.grid_cluster, nn/pool/voxel_grid.py:66).
+ * pos [n, d] row-major, size / start / end [d], all val_dtype (B200MP_F32 or B200MP_F64).  out [n] int64 gets
+ * sum_k trunc((pos[i, k] - start[k]) / size[k]) * prod_{k' < k} (trunc((end[k'] - start[k']) / size[k']) + 1), one IEEE
+ * subtract and one IEEE divide per term in val_dtype, converted toward zero (saturating, NaN -> INT64_MIN) and summed
+ * with 64-bit wrap-around.  A NULL start / end is the column min / max of pos (NaN propagating), computed on the device
+ * into ws, which then holds 514 d elements of val_dtype.  1 <= d <= 65535. */
+int b200mp_grid_cluster(const void* pos, const void* size, const void* start, const void* end, int64_t n, int64_t d,
+                        int64_t* out, void* ws, int val_dtype, void* stream);
 
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)
  * out[index[e], :] (+)= src[e, :] for an UNSORTED index.  Replaces utils/_scatter.py:14-138

@@ -3,4 +3,4 @@ from .aggr import (Aggregation, FusedAggregation, MaxAggregation, MeanAggregatio
                    StdAggregation, SumAggregation, VarAggregation, aggregation_resolver)
 from .conv import (CGConv, FastRGCNConv, GATConv, GATv2Conv, GCNConv, GENConv, GINConv, GINEConv, GraphConv, HeteroLinear,  # noqa: F401
                    NNConv, PNAConv, ResGatedGraphConv, RGCNConv, SAGEConv, SplineConv, TransformerConv)
-from .pool import fps, knn, knn_graph, nearest, radius, radius_graph  # noqa: F401
+from .pool import fps, graclus, knn, knn_graph, nearest, radius, radius_graph, voxel_grid  # noqa: F401

@@ -1,5 +1,6 @@
-"""Graph construction on point clouds: mirrors of torch_geometric.nn.{fps, knn, knn_graph, radius, radius_graph,
-nearest} (nn/pool/__init__.py:41-375) on the sm_90a kernels of csrc/point.cu.
+"""Graph construction on point clouds and cluster vectors for pooling: mirrors of torch_geometric.nn.{fps, knn,
+knn_graph, radius, radius_graph, nearest} (nn/pool/__init__.py:41-375) on the sm_90a kernels of csrc/point.cu, and of
+graclus and voxel_grid (nn/pool/graclus.py, nn/pool/voxel_grid.py) on those of csrc/cluster.cu.
 
 Signatures, defaults, `flow` and `loop` handling and `batch_size` are the reference's; `num_workers` is accepted and
 ignored, as the reference documents for inputs on the GPU.  Inputs are CUDA float32 / bfloat16 tensors (CPU, float16
@@ -76,4 +77,46 @@ def nearest(x: Tensor, y: Tensor, batch_x: Optional[Tensor] = None, batch_y: Opt
     return ops.nearest(x, y, _batch_to_ptr(batch_x), _batch_to_ptr(batch_y))
 
 
-__all__ = ['fps', 'knn', 'knn_graph', 'radius', 'radius_graph', 'nearest']
+def graclus(edge_index: Tensor, weight: Optional[Tensor] = None, num_nodes: Optional[int] = None) -> Tensor:
+    """Greedy matching of the graph (nn/pool/graclus.py:12-39): the edges sorted by source, then ops.graclus on the
+    CSR adjacency.  Returns the cluster vector: min(u, v) for each matched pair, u for each singleton.  The colouring
+    seed is drawn from torch's CPU generator."""
+    if num_nodes is None:
+        num_nodes = int(edge_index.max()) + 1 if edge_index.numel() > 0 else 0
+    row, col = edge_index[0], edge_index[1]
+    # sort_edge_index's order: by row, then by column (a stable sort of the key row * N + col)
+    perm = torch.sort(row.long() * num_nodes + col.long(), stable=True)[1]
+    row, col = row[perm], col[perm]
+    weight = None if weight is None else weight[perm]
+    return ops.graclus(ops.index2ptr(row, num_nodes), col, weight)
+
+
+def _coords(v, dim: int, like: Tensor) -> Tensor:
+    """The reference's `repeat(v, dim)` of a number, list or tensor, as a tensor of like's dtype and device."""
+    if not isinstance(v, Tensor):
+        v = torch.tensor(v, dtype=like.dtype, device=like.device)
+    v = v.reshape(-1)
+    if v.numel() == 1:
+        return v.repeat(dim)
+    if v.numel() >= dim:
+        return v[:dim]
+    return torch.cat([v, v[-1:].repeat(dim - v.numel())])
+
+
+def voxel_grid(pos: Tensor, size, batch: Optional[Tensor] = None, start=None, end=None) -> Tensor:
+    """Voxel grid pooling's cluster vector (nn/pool/voxel_grid.py:9-66): the batch index is appended to pos as one more
+    coordinate of voxel size 1 (start 0, end batch.max()), then ops.grid_cluster.  pos is CUDA float32 / float64."""
+    pos = pos.unsqueeze(-1) if pos.dim() == 1 else pos
+    dim = pos.size(1)
+    if batch is None:
+        batch = pos.new_zeros(pos.size(0), dtype=torch.long)
+    pos = torch.cat([pos, batch.view(-1, 1).to(pos.dtype)], dim=-1)
+    size = torch.cat([_coords(size, dim, pos), pos.new_ones(1)])
+    if start is not None:
+        start = torch.cat([_coords(start, dim, pos), pos.new_zeros(1)])
+    if end is not None:
+        end = torch.cat([_coords(end, dim, pos), batch.max().unsqueeze(0).to(pos.dtype)])
+    return ops.grid_cluster(pos, size, start, end)
+
+
+__all__ = ['fps', 'knn', 'knn_graph', 'radius', 'radius_graph', 'nearest', 'graclus', 'voxel_grid']

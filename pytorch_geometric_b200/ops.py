@@ -14,7 +14,7 @@ from torch import Tensor
 
 from ._lib import check, lib
 
-F32, BF16 = 0, 1
+F32, BF16, F64 = 0, 1, 2
 I32, I64 = 0, 1
 REDUCE = {"sum": 0, "add": 0, "mean": 1, "min": 2, "amin": 2, "max": 3, "amax": 3, "mul": 4}
 
@@ -962,6 +962,91 @@ def fps(src: Tensor, ptr: Optional[Tensor] = None, ratio: float = 0.5, random_st
     dist = torch.empty(N, dtype=torch.float32, device=src.device)
     _timed("fps", 1, lib().b200mp_fps, _p(src), _p(ptr), N, src.size(1), _np(ptr), _p(rnd), _p(offsets), _p(dist),
            _p(out), _vdt(src), pdt, _stream())
+    return out
+
+
+# ------------------------------------------------------------------ clustering for pooling (csrc/cluster.cu)
+GRACLUS_MAX_ROUNDS = 256
+_GRACLUS_WEIGHTS = {torch.float32: F32, torch.bfloat16: BF16, torch.float64: F64}
+
+
+def graclus(rowptr: Tensor, col: Tensor, weight: Optional[Tensor] = None, seed: Optional[int] = None,
+            return_rounds: bool = False):
+    """[N] int64 cluster vector of a greedy matching of the CSR graph (rowptr [N + 1], col): min(u, v) for each
+    matched pair, u for each singleton (pyg_lib.ops.graclus_cluster; csrc/cluster.cu states the rules).  weight (one
+    float32 / bfloat16 / float64 value per CSR entry) makes each node pick its heaviest eligible neighbour.  The result
+    is a pure function of (graph, weight, seed); seed defaults to a draw from torch's CPU generator, so it is
+    reproducible under torch.manual_seed and costs no device synchronisation.  return_rounds also returns the number
+    of matching rounds as a 0-dim int32 CUDA tensor (at most GRACLUS_MAX_ROUNDS)."""
+    _cuda(rowptr, col, weight)
+    idt = _same_idx(rowptr, col)
+    if rowptr.dim() != 1 or rowptr.numel() < 1 or col.dim() != 1:
+        raise ValueError(f"rowptr must be [N + 1] and col [E], got {tuple(rowptr.shape)} and {tuple(col.shape)}")
+    n = rowptr.numel() - 1
+    if n >= 2**31 - 1:
+        raise ValueError(f"graclus takes fewer than 2^31 - 1 nodes, got {n}")
+    wdt = F32
+    if weight is not None:
+        if weight.dtype not in _GRACLUS_WEIGHTS:
+            raise TypeError(f"graclus weights must be float32, bfloat16 or float64, got {weight.dtype}")
+        if weight.numel() != col.numel() or weight.device != col.device:
+            raise ValueError(f"weight must hold one value per edge on {col.device}, got {weight.numel()} for "
+                             f"{col.numel()} edges on {weight.device}")
+        wdt = _GRACLUS_WEIGHTS[weight.dtype]
+        weight = weight.detach().reshape(-1).contiguous()
+    if rowptr.device != col.device:
+        raise RuntimeError(f"rowptr and col must share a device, got {rowptr.device} and {col.device}")
+    rowptr, col = rowptr.contiguous(), col.contiguous()
+    from . import _debug
+    if _debug.enabled() and n > 0:
+        rp, c = rowptr.cpu(), col.cpu()
+        if int(rp[0]) != 0 or int(rp[-1]) != c.numel() or bool((rp[1:] < rp[:-1]).any()):
+            raise ValueError(f"rowptr must be non-decreasing from 0 to the number of edges {c.numel()}")
+        if c.numel() > 0 and (int(c.min()) < 0 or int(c.max()) >= n):
+            raise IndexError(f"col must hold node indices in [0, {n})")
+    if seed is None:
+        seed = int(torch.randint(0, 2**63 - 1, (), dtype=torch.int64))
+    seed = int(seed) & (2**64 - 1)
+    cluster = torch.empty(n, dtype=torch.int64, device=rowptr.device)
+    ws = torch.empty(2 * n + 3, dtype=torch.int32, device=rowptr.device)
+    _timed("graclus", 1 if n > 0 else 0, lib().b200mp_graclus, _p(rowptr), _p(col), _p(weight), n, seed, _p(cluster),
+           _p(ws), idt, wdt, _stream())
+    return (cluster, ws[2 * n + 2]) if return_rounds else cluster
+
+
+def grid_cluster(pos: Tensor, size: Tensor, start: Optional[Tensor] = None, end: Optional[Tensor] = None) -> Tensor:
+    """[N] int64 voxel index of each point (pyg_lib.ops.grid_cluster): sum_d trunc((pos[i, d] - start[d]) / size[d])
+    * prod_{d' < d} (trunc((end[d'] - start[d']) / size[d']) + 1) in pos's dtype (float32 or float64).  A missing
+    start / end is the column min / max of pos (NaN propagating), computed on the device.  size, start and end hold D
+    values and are cast to pos's dtype."""
+    _cuda(pos, size, start, end)
+    if pos.dtype in (torch.float16, torch.bfloat16):
+        raise TypeError(f"grid_cluster takes float32 or float64 positions, got {pos.dtype}: voxel_grid appends the "
+                        "batch index as a coordinate, which stops being exact above 2048 (float16) or 256 (bfloat16)")
+    if pos.dtype not in (torch.float32, torch.float64):
+        raise TypeError(f"grid_cluster takes float32 or float64 positions, got {pos.dtype}")
+    pos = pos.detach()
+    pos = (pos.view(-1, 1) if pos.dim() == 1 else pos.flatten(1)).contiguous()
+    n, d = pos.shape
+    if not 1 <= d <= 65535:
+        raise ValueError(f"grid_cluster takes 1 to 65535 coordinates per point, got {d}")
+
+    def vec(t: Optional[Tensor], name: str) -> Optional[Tensor]:
+        if t is None:
+            return None
+        if t.device != pos.device:
+            raise RuntimeError(f"{name} must be on the points' device {pos.device}, got {t.device}")
+        t = t.detach().to(pos.dtype).reshape(-1).contiguous()
+        if t.numel() != d:
+            raise ValueError(f"{name} must hold one value per coordinate ({d}), got {t.numel()}")
+        return t
+
+    size, start, end = vec(size, "size"), vec(start, "start"), vec(end, "end")
+    out = torch.empty(n, dtype=torch.int64, device=pos.device)
+    ws = torch.empty(514 * d, dtype=pos.dtype, device=pos.device) if start is None or end is None else None
+    n_kernels = 0 if n == 0 else (1 if ws is None else 3)
+    _timed("grid_cluster", n_kernels, lib().b200mp_grid_cluster, _p(pos), _p(size), _p(start), _p(end), n, d, _p(out),
+           _p(ws), F64 if pos.dtype == torch.float64 else F32, _stream())
     return out
 
 

@@ -129,6 +129,8 @@ def install(layers: bool = False, extensions: bool = True, flip_flags: bool = Fa
         counts["spline_ops"] = k
         # the point-cloud functions and DynamicEdgeConv / GravNetConv / XConv call torch.ops.pyg.* directly
         counts["point_ops"] = shims.register_point_ops()
+        # graclus and voxel_grid call torch.ops.pyg.graclus_cluster / grid_cluster directly
+        counts["cluster_ops"] = shims.register_cluster_ops()
         if flip_flags:
             for flag in ("WITH_TORCH_SCATTER", "WITH_SOFTMAX", "WITH_INDEX_SORT", "WITH_SEGMM", "WITH_GMM"):
                 _set(tg_typing, flag, True)
@@ -138,6 +140,9 @@ def install(layers: bool = False, extensions: bool = True, flip_flags: bool = Fa
             for flag in ("WITH_KNN", "WITH_RADIUS", "WITH_FPS", "WITH_NEAREST"):
                 _set(tg_typing, flag, True)
             counts["point_flags"] = 4
+            for flag in ("WITH_GRACLUS", "WITH_GRID_CLUSTER"):
+                _set(tg_typing, flag, True)
+            counts["cluster_flags"] = 2
 
     if layers:
         import torch_geometric.nn as tgnn

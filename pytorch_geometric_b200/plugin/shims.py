@@ -15,9 +15,12 @@ engine: flipping `torch_geometric.typing.WITH_*` to True with these modules boun
   pyg_lib.ops.spline_weighting(x, weight, basis, weight_index)                     nn/conv/spline_conv.py:153
   torch.ops.pyg.knn / radius / fps / nearest (also pyg_lib.ops.*)                  nn/pool/__init__.py:85-375,
                                                                                    nn/conv/{edge,gravnet,x}_conv.py
+  torch.ops.pyg.graclus_cluster / grid_cluster (also pyg_lib.ops.*)               nn/pool/graclus.py:39,
+                                                                                   nn/pool/voxel_grid.py:66
 
 CUDA fp32 / bf16 operands run in the engine.  The spline and point-cloud ops have no reference fall-back (the reference has no
-ATen branch for them), so CPU, float16 and float64 operands raise RuntimeError.  Other CPU operands fall through to the reference's own ATen branch (the
+ATen branch for them), so CPU, float16 and float64 operands raise RuntimeError; neither have the clustering ops, which
+take CUDA tensors only (graclus: float32 / bfloat16 / float64 weights; grid_cluster: float32 / float64 positions).  Other CPU operands fall through to the reference's own ATen branch (the
 shim calls the reference function with the extension flag switched off for the duration of the call) -- the engine
 itself never computes on the CPU.  torch.ops.torch_sparse.* are `torch.library` operators with a CUDA implementation,
 a Meta (shape) implementation so tracing stays legal, and autograd formulas that use the transposed structure the
@@ -327,25 +330,59 @@ def _pyg_nearest(x: Tensor, y: Tensor, ptr_x: Optional[Tensor] = None, ptr_y: Op
 POINT_OPS = {"knn": _pyg_knn, "radius": _pyg_radius, "fps": _pyg_fps, "nearest": _pyg_nearest}
 
 
-def register_point_ops() -> int:
-    """Defines torch.ops.pyg.{knn, radius, fps, nearest} with pyg-lib's schemas and CUDA implementations only.  Returns
-    the number of operators this call or an earlier one defined; an operator the namespace already has (the real
-    pyg-lib is installed) is left alone."""
-    global _POINT_LIB
-    if _POINT_LIB is not None:
-        return _POINT_LIB[1]
+def _define_pyg_ops(schemas: dict, impls: dict) -> tuple:
+    """Defines the torch.ops.pyg operators of `schemas` that the namespace lacks, with CUDA implementations only (an
+    operator it already has -- the real pyg-lib is installed -- is left alone).  Returns (library, number defined)."""
     missing = []
-    for name in POINT_SCHEMAS:
+    for name in schemas:
         try:
             getattr(torch.ops.pyg, name)
         except (AttributeError, RuntimeError):
             missing.append(name)
     lib = torch.library.Library("pyg", "FRAGMENT")
     for name in missing:
-        lib.define(POINT_SCHEMAS[name])
-        lib.impl(name, POINT_OPS[name], "CUDA")
-    _POINT_LIB = (lib, len(missing))
-    return len(missing)
+        lib.define(schemas[name])
+        lib.impl(name, impls[name], "CUDA")
+    return lib, len(missing)
+
+
+def register_point_ops() -> int:
+    """Defines torch.ops.pyg.{knn, radius, fps, nearest} with pyg-lib's schemas and CUDA implementations only.  Returns
+    the number of operators this call or an earlier one defined; an operator the namespace already has (the real
+    pyg-lib is installed) is left alone."""
+    global _POINT_LIB
+    if _POINT_LIB is None:
+        _POINT_LIB = _define_pyg_ops(POINT_SCHEMAS, POINT_OPS)
+    return _POINT_LIB[1]
+
+
+# ================================================================================================ torch.ops.pyg (clustering)
+_CLUSTER_LIB = None
+CLUSTER_SCHEMAS = {
+    "graclus_cluster": "graclus_cluster(Tensor rowptr, Tensor col, Tensor? weight) -> Tensor",
+    "grid_cluster": "grid_cluster(Tensor pos, Tensor size, Tensor? start, Tensor? end) -> Tensor",
+}
+
+
+def _pyg_graclus_cluster(rowptr: Tensor, col: Tensor, weight: Optional[Tensor] = None) -> Tensor:
+    return ops.graclus(rowptr, col, weight)
+
+
+def _pyg_grid_cluster(pos: Tensor, size: Tensor, start: Optional[Tensor] = None,
+                      end: Optional[Tensor] = None) -> Tensor:
+    return ops.grid_cluster(pos, size, start, end)
+
+
+CLUSTER_OPS = {"graclus_cluster": _pyg_graclus_cluster, "grid_cluster": _pyg_grid_cluster}
+
+
+def register_cluster_ops() -> int:
+    """Defines torch.ops.pyg.{graclus_cluster, grid_cluster} with pyg-lib's schemas and CUDA implementations only, as
+    register_point_ops does for the point-cloud operators."""
+    global _CLUSTER_LIB
+    if _CLUSTER_LIB is None:
+        _CLUSTER_LIB = _define_pyg_ops(CLUSTER_SCHEMAS, CLUSTER_OPS)
+    return _CLUSTER_LIB[1]
 
 
 def pyg_lib_module() -> types.ModuleType:
@@ -362,5 +399,7 @@ def pyg_lib_module() -> types.ModuleType:
     m.ops.radius = _pyg_radius
     m.ops.fps = _pyg_fps
     m.ops.nearest = _pyg_nearest
+    m.ops.graclus_cluster = _pyg_graclus_cluster
+    m.ops.grid_cluster = _pyg_grid_cluster
     m.__version__ = "b200mp-shim"
     return m

@@ -633,6 +633,22 @@ int b200mp_graclus(const void* rowptr, const void* col, const void* weight, int6
 int b200mp_grid_cluster(const void* pos, const void* size, const void* start, const void* end, int64_t n, int64_t d,
                         int64_t* out, void* ws, int val_dtype, void* stream);
 
+/* ------------------------------------------------------------------ random walks (uniform and node2vec)
+ * Replaces pyg_lib.ops.random_walk (torch.ops.pyg.random_walk: nn/models/node2vec.py:64,103, utils/dropout.py:285,
+ * transforms/rooted_subgraph.py:171).  rowptr [n + 1] / col [n_edges] is the CSR adjacency, start [n_walks] the first
+ * node of each walk, all idx_dtype; n < 2^31 - 1.  out [n_walks, walk_length + 1] (idx_dtype) gets each walk, column 0
+ * being start.  p, q: finite and > 0; p = q = 1 gives uniform walks, anything else node2vec's second-order walk by
+ * rejection sampling with at most max_trials trials per step before an exact draw.  The walks are a pure function of
+ * (graph, start, walk_length, p, q, max_trials, seed); csrc/random_walk.cu states the generator and every rule.  A start
+ * outside [0, n) gives a row of -1; a picked node outside [0, n) (or a row with bounds outside [0, n_edges]) ends its
+ * walk, the rest of the row being -1.  rows_unsorted [1] int32 (DEVICE; required when p != 1 or q != 1) is 1 when
+ * some row of col decreases, which selects a linear scan over a binary search for the neighbour test; with
+ * refresh_rows_unsorted it is computed here first (O(n_edges)), otherwise it is read as the caller left it.
+ * n_walks = 0 launches nothing. */
+int b200mp_random_walk(const void* rowptr, const void* col, const void* start, int64_t n, int64_t n_edges,
+                       int64_t n_walks, int64_t walk_length, double p, double q, int64_t max_trials, uint64_t seed,
+                       int32_t* rows_unsorted, int refresh_rows_unsorted, void* out, int idx_dtype, void* stream);
+
 /* ------------------------------------------------------------------ COO scatter fallback (atomics)
  * out[index[e], :] (+)= src[e, :] for an UNSORTED index.  Replaces utils/_scatter.py:14-138
  * (aten::scatter_add_ / scatter_reduce_, torch_scatter.scatter).  fp32 only.  `count` is a

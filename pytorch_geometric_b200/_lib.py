@@ -95,6 +95,7 @@ _SIGS = {
     "b200mp_fps": (_INT, [_P, _P, _I64, _I64, _I64, _P, _P, _P, _P, _INT, _INT, _P]),
     "b200mp_graclus": (_INT, [_P, _P, _P, _I64, _U64, _P, _P, _INT, _INT, _P]),
     "b200mp_grid_cluster": (_INT, [_P] * 4 + [_I64, _I64, _P, _P, _INT, _P]),
+    "b200mp_random_walk": (_INT, [_P] * 3 + [_I64] * 4 + [_D, _D, _I64, _U64, _P, _INT, _P, _INT, _P]),
     "b200mp_scatter_coo": (_INT, [_P, _P, _P, _P, _I64, _I64, _I64, _INT, _INT, _P]),
     "b200mp_split_tf32": (_INT, [_P, _P, _P, _I64, _P]),
     "b200mp_split_tf32_transposed": (_INT, [_P, _P, _P, _I64, _I64, _P]),

@@ -65,15 +65,11 @@ struct GcArgs {
     int32_t* rounds;     // [1]: rounds used
 };
 
-// splitmix64's finaliser on seed + key * golden ratio, as attention dropout (attention.cu) hashes its slots.
+// splitmix64's finaliser on seed + key * golden ratio (common.cuh), as attention dropout (attention.cu) hashes its slots.
 __device__ __forceinline__ bool gc_blue(unsigned long long seed, int round, int64_t n, int64_t u) {
     const unsigned long long key =
         static_cast<unsigned long long>(round) * static_cast<unsigned long long>(n) + static_cast<unsigned long long>(u);
-    unsigned long long z = seed + key * 0x9E3779B97F4A7C15ull;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    z ^= z >> 31;
-    return (z >> 63) != 0ull;
+    return (splitmix64(seed, key) >> 63) != 0ull;
 }
 
 __device__ __forceinline__ double gc_weight(const float* w, int64_t e) { return static_cast<double>(__ldg(w + e)); }

@@ -213,4 +213,13 @@ __device__ __forceinline__ I ldg_idx(const I* p) {
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+// splitmix64's finaliser on seed + key * golden ratio (mod 2^64): the counter-based generator of graclus's colours
+// (cluster.cu) and of the random walks' draws (random_walk.cu).
+__device__ __forceinline__ unsigned long long splitmix64(unsigned long long seed, unsigned long long key) {
+    unsigned long long z = seed + key * 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
 }  // namespace b200mp

@@ -7,6 +7,8 @@ no CPU fallback.
 from __future__ import annotations
 
 import ctypes
+import math
+from collections import OrderedDict
 from typing import Optional, Tuple
 
 import torch
@@ -1047,6 +1049,86 @@ def grid_cluster(pos: Tensor, size: Tensor, start: Optional[Tensor] = None, end:
     n_kernels = 0 if n == 0 else (1 if ws is None else 3)
     _timed("grid_cluster", n_kernels, lib().b200mp_grid_cluster, _p(pos), _p(size), _p(start), _p(end), n, d, _p(out),
            _p(ws), F64 if pos.dtype == torch.float64 else F32, _stream())
+    return out
+
+
+# ------------------------------------------------------------------ random walks (csrc/random_walk.cu)
+# Trials per node2vec step before the exact draw, which scans the current row (twice, with a neighbour test per entry).
+# A walk's stationary distribution favours hubs, so with 64 trials (a rejection chance of up to (15/16)^64 = 1.6 %
+# at p = 1/4, q = 4) the exact draw often lands on rows of millions of entries; 1024 makes it negligible for moderate
+# p and q and still bounds the work for extreme ones (README: the row_order lines).
+RANDOM_WALK_MAX_TRIALS = 1024
+_ROWS_UNSORTED = OrderedDict()       # (rowptr, col) identity -> (rowptr, col, versions, rows_unsorted flag [1] int32)
+_ROWS_UNSORTED_ENTRIES = 8
+
+
+def _rows_unsorted_flag(rowptr: Tensor, col: Tensor) -> Tuple[Tensor, bool]:
+    """The device flag of the neighbour test (1 when some row of col decreases) and whether it must be computed: cached
+    by the identity and version of both tensors, the strong references living in the cache entry (as plugin/graphs.py
+    caches pair graphs), so repeated batches over one graph check it once."""
+    key = (rowptr.data_ptr(), col.data_ptr(), rowptr.numel(), col.numel(), rowptr.dtype, rowptr.device)
+    hit = _ROWS_UNSORTED.get(key)
+    if hit is not None and hit[2] == (rowptr._version, col._version):
+        _ROWS_UNSORTED.move_to_end(key)
+        return hit[3], False
+    flag = torch.empty(1, dtype=torch.int32, device=rowptr.device)
+    _ROWS_UNSORTED[key] = (rowptr, col, (rowptr._version, col._version), flag)
+    while len(_ROWS_UNSORTED) > _ROWS_UNSORTED_ENTRIES:
+        _ROWS_UNSORTED.popitem(last=False)
+    return flag, True
+
+
+def random_walk(rowptr: Tensor, col: Tensor, start: Tensor, walk_length: int, p: float = 1.0, q: float = 1.0,
+                seed: Optional[int] = None, max_trials: int = RANDOM_WALK_MAX_TRIALS) -> Tensor:
+    """[S, walk_length + 1] random walks over the CSR graph (rowptr [N + 1], col [E]) from each node of start [S], in
+    the index dtype (pyg_lib.ops.random_walk; csrc/random_walk.cu states the rules).  p = q = 1 gives uniform walks;
+    other values give node2vec's second-order walks (return parameter p, in-out parameter q) by rejection sampling,
+    with an exact draw after max_trials rejected trials of a step.  A node without out-edges keeps the walk where it
+    is.  A start outside [0, N) gives a row of -1, and a column value outside [0, N) ends its walk with -1s (debug mode
+    raises instead).  The walks are a pure function of (graph, start, walk_length, p, q, max_trials, seed); seed
+    defaults to a draw from torch's CPU generator, so torch.manual_seed reproduces them and nothing synchronises."""
+    _cuda(rowptr, col, start)
+    idt = _same_idx(rowptr, col, start)
+    if rowptr.dim() != 1 or rowptr.numel() < 1 or col.dim() != 1 or start.dim() != 1:
+        raise ValueError(f"rowptr must be [N + 1], col [E] and start [S], got {tuple(rowptr.shape)}, "
+                         f"{tuple(col.shape)} and {tuple(start.shape)}")
+    if not (rowptr.device == col.device == start.device):
+        raise RuntimeError(f"rowptr, col and start must share a device, got {rowptr.device}, {col.device} and "
+                           f"{start.device}")
+    walk_length, p, q, max_trials = int(walk_length), float(p), float(q), int(max_trials)
+    if walk_length < 0:
+        raise ValueError(f"random_walk takes walk_length >= 0, got {walk_length}")
+    for name, v in (("p", p), ("q", q)):
+        if not (math.isfinite(v) and v > 0.0):
+            raise ValueError(f"random_walk takes a finite {name} > 0, got {v}")
+    if max_trials < 0:
+        raise ValueError(f"random_walk takes max_trials >= 0, got {max_trials}")
+    n = rowptr.numel() - 1
+    if n >= 2**31 - 1:
+        raise ValueError(f"random_walk takes fewer than 2^31 - 1 nodes, got {n}")
+    rowptr, col, start = rowptr.contiguous(), col.contiguous(), start.contiguous()
+    from . import _debug
+    if _debug.enabled():
+        rp, c, s = rowptr.cpu(), col.cpu(), start.cpu()
+        if int(rp[0]) != 0 or int(rp[-1]) != c.numel() or bool((rp[1:] < rp[:-1]).any()):
+            raise ValueError(f"rowptr must be non-decreasing from 0 to the number of edges {c.numel()}")
+        if c.numel() > 0 and (int(c.min()) < 0 or int(c.max()) >= n):
+            raise IndexError(f"col must hold node indices in [0, {n})")
+        if s.numel() > 0 and (int(s.min()) < 0 or int(s.max()) >= n):
+            raise IndexError(f"start must hold node indices in [0, {n})")
+    S = start.numel()
+    out = torch.empty(S, walk_length + 1, dtype=rowptr.dtype, device=rowptr.device)
+    if S == 0:
+        return out
+    if seed is None:
+        seed = int(torch.randint(0, 2**63 - 1, (), dtype=torch.int64))
+    seed = int(seed) & (2**64 - 1)
+    flag, refresh = None, False
+    if p != 1.0 or q != 1.0:
+        flag, refresh = _rows_unsorted_flag(rowptr, col)
+    n_kernels = 1 + int(refresh and n > 0 and col.numel() > 1)
+    _timed("random_walk", n_kernels, lib().b200mp_random_walk, _p(rowptr), _p(col), _p(start), n, col.numel(), S,
+           walk_length, p, q, max_trials, seed, _p(flag), int(refresh), _p(out), idt, _stream())
     return out
 
 

@@ -13,6 +13,7 @@ The reference has no FFI; it late-binds Python callables and a handful of option
                     the `WITH_*` switches are turned on so the reference's own extension branches run them  -> shims.py
   (4) layers        subclasses of the reference's layer classes with fully fused `forward` / `message_and_aggregate`
                     (`pytorch_geometric_b200.plugin.conv`); `layers=True` rebinds `torch_geometric.nn.<Layer>`      -> conv.py
+                    and `torch_geometric.nn.Node2Vec` to a subclass whose graph moves to the GPU with it      -> models.py
 
 CPU tensors, unsupported dtypes and `torch.compile` tracing (`is_compiling()`, as the reference gates its own
 extension calls: utils/_scatter.py:85,120) fall through to the untouched reference code.
@@ -131,6 +132,8 @@ def install(layers: bool = False, extensions: bool = True, flip_flags: bool = Fa
         counts["point_ops"] = shims.register_point_ops()
         # graclus and voxel_grid call torch.ops.pyg.graclus_cluster / grid_cluster directly
         counts["cluster_ops"] = shims.register_cluster_ops()
+        # Node2Vec, dropout_path and RootedRWSubgraph call torch.ops.pyg.random_walk directly
+        counts["walk_ops"] = shims.register_walk_ops()
         if flip_flags:
             for flag in ("WITH_TORCH_SCATTER", "WITH_SOFTMAX", "WITH_INDEX_SORT", "WITH_SEGMM", "WITH_GMM"):
                 _set(tg_typing, flag, True)
@@ -143,6 +146,14 @@ def install(layers: bool = False, extensions: bool = True, flip_flags: bool = Fa
             for flag in ("WITH_GRACLUS", "WITH_GRID_CLUSTER"):
                 _set(tg_typing, flag, True)
             counts["cluster_flags"] = 2
+            # Node2Vec and dropout_path gate on WITH_PYG_LIB, which NeighborLoader and to_hetero read too: the global
+            # stays off (the engine has no neighbour sampler); node2vec's own binding of it is set, and dropout_path
+            # is wrapped to switch it on for its own call only
+            import torch_geometric.nn.models.node2vec as tg_node2vec
+            from torch_geometric.utils import dropout as tg_dropout
+            _set(tg_node2vec, "WITH_PYG_LIB", True)
+            theirs = tg_dropout.dropout_path
+            counts["walk_flags"] = 1 + _rebind_everywhere("dropout_path", theirs, shims.make_dropout_path(theirs))
 
     if layers:
         import torch_geometric.nn as tgnn
@@ -156,6 +167,16 @@ def install(layers: bool = False, extensions: bool = True, flip_flags: bool = Fa
                     _set(mod, cls, getattr(ours_conv, sub))
                     k += 1
         counts["layers"] = k
+        # Node2Vec keeps its graph in buffers that follow the module to the GPU (models.py)
+        import torch_geometric.nn.models as tgmodels
+
+        from .models import B200Node2Vec
+        k = 0
+        for mod in (tgnn, tgmodels):
+            if hasattr(mod, "Node2Vec"):
+                _set(mod, "Node2Vec", B200Node2Vec)
+                k += 1
+        counts["models"] = k
     return counts
 
 

@@ -17,10 +17,14 @@ engine: flipping `torch_geometric.typing.WITH_*` to True with these modules boun
                                                                                    nn/conv/{edge,gravnet,x}_conv.py
   torch.ops.pyg.graclus_cluster / grid_cluster (also pyg_lib.ops.*)               nn/pool/graclus.py:39,
                                                                                    nn/pool/voxel_grid.py:66
+  torch.ops.pyg.random_walk(rowptr, col, seed, walk_length, p, q) (also pyg_lib.ops.*)   nn/models/node2vec.py:64,103,
+                                                                                   utils/dropout.py:285,
+                                                                                   transforms/rooted_subgraph.py:171
 
 CUDA fp32 / bf16 operands run in the engine.  The spline and point-cloud ops have no reference fall-back (the reference has no
 ATen branch for them), so CPU, float16 and float64 operands raise RuntimeError; neither have the clustering ops, which
-take CUDA tensors only (graclus: float32 / bfloat16 / float64 weights; grid_cluster: float32 / float64 positions).  Other CPU operands fall through to the reference's own ATen branch (the
+take CUDA tensors only (graclus: float32 / bfloat16 / float64 weights; grid_cluster: float32 / float64 positions), nor
+has random_walk (int32 or int64 indices).  Other CPU operands fall through to the reference's own ATen branch (the
 shim calls the reference function with the extension flag switched off for the duration of the call) -- the engine
 itself never computes on the CPU.  torch.ops.torch_sparse.* are `torch.library` operators with a CUDA implementation,
 a Meta (shape) implementation so tracing stays legal, and autograd formulas that use the transposed structure the
@@ -52,16 +56,24 @@ def _ok(t) -> bool:
 
 
 @contextlib.contextmanager
-def _flags_off(*names):
+def _flags_set(value: bool, *names):
     import torch_geometric.typing as T
     old = {n: getattr(T, n) for n in names}
     try:
         for n in names:
-            setattr(T, n, False)
+            setattr(T, n, value)
         yield
     finally:
         for n, v in old.items():
             setattr(T, n, v)
+
+
+def _flags_off(*names):
+    return _flags_set(False, *names)
+
+
+def _flags_on(*names):
+    return _flags_set(True, *names)
 
 
 # ================================================================================================ torch_scatter
@@ -385,6 +397,49 @@ def register_cluster_ops() -> int:
     return _CLUSTER_LIB[1]
 
 
+# ================================================================================================ torch.ops.pyg (random walks)
+_WALK_LIB = None
+WALK_SCHEMAS = {
+    "random_walk": "random_walk(Tensor rowptr, Tensor col, Tensor seed, int walk_length, float p=1.0, "
+                   "float q=1.0) -> Tensor",
+}
+
+
+def _pyg_random_walk(rowptr: Tensor, col: Tensor, seed: Tensor, walk_length: int, p: float = 1.0,
+                     q: float = 1.0) -> Tensor:
+    # pyg-lib names the start nodes `seed`; the walks' random seed comes from torch's CPU generator
+    return ops.random_walk(rowptr, col, seed, walk_length, p, q)
+
+
+WALK_OPS = {"random_walk": _pyg_random_walk}
+
+
+def register_walk_ops() -> int:
+    """Defines torch.ops.pyg.random_walk with pyg-lib's schema and a CUDA implementation only, as register_point_ops
+    does for the point-cloud operators."""
+    global _WALK_LIB
+    if _WALK_LIB is None:
+        _WALK_LIB = _define_pyg_ops(WALK_SCHEMAS, WALK_OPS)
+    return _WALK_LIB[1]
+
+
+def make_dropout_path(theirs):
+    """utils.dropout_path (utils/dropout.py:221-298) for CUDA edge_index: the unmodified reference function with the
+    global WITH_PYG_LIB switched on for this call only, so it reaches torch.ops.pyg.random_walk.  The flag itself stays
+    off: NeighborLoader and to_hetero read it too, and the engine has no neighbour sampler.  CPU input goes to the
+    reference unchanged (and raises its own ImportError)."""
+    import functools
+
+    @functools.wraps(theirs)
+    def dropout_path(edge_index: Tensor, p: float = 0.2, walks_per_node: int = 1, walk_length: int = 3,
+                     num_nodes: Optional[int] = None, is_sorted: bool = False, training: bool = True):
+        if isinstance(edge_index, Tensor) and edge_index.is_cuda:
+            with _flags_on("WITH_PYG_LIB"):
+                return theirs(edge_index, p, walks_per_node, walk_length, num_nodes, is_sorted, training)
+        return theirs(edge_index, p, walks_per_node, walk_length, num_nodes, is_sorted, training)
+    return dropout_path
+
+
 def pyg_lib_module() -> types.ModuleType:
     m = types.ModuleType("pyg_lib")
     m.__doc__ = "pytorch_geometric_b200 shim of the pyg_lib.ops operators on the aggregation path"
@@ -401,5 +456,6 @@ def pyg_lib_module() -> types.ModuleType:
     m.ops.nearest = _pyg_nearest
     m.ops.graclus_cluster = _pyg_graclus_cluster
     m.ops.grid_cluster = _pyg_grid_cluster
+    m.ops.random_walk = _pyg_random_walk
     m.__version__ = "b200mp-shim"
     return m

@@ -166,6 +166,43 @@ def index_sort(inputs: Tensor, max_value: Optional[int] = None, stable: bool = F
     return ks, perm.to(torch.int64)
 
 
+def sort_edge_index_by_row_col(edge_index: Tensor, num_nodes: int) -> Tuple[Tensor, Tensor, Tensor]:
+    """(row, col, perm): the edges ordered by row, then column, as torch_geometric.utils.sort_edge_index orders them
+    (utils/_sort_edge_index.py: the key row * N + col), by two stable passes of the engine's sort with keys in [0, N)."""
+    row, col = edge_index[0].contiguous(), edge_index[1].contiguous()
+    _, by_col, _ = ops.sort_by_key(col, num_nodes, want_sorted=False, want_ptr=False)
+    _, by_row, _ = ops.sort_by_key(row[by_col], num_nodes, want_sorted=False, want_ptr=False)
+    perm = by_col[by_row]
+    return row[perm], col[perm], perm
+
+
+def dropout_path(edge_index: Tensor, p: float = 0.2, walks_per_node: int = 1, walk_length: int = 3,
+                 num_nodes: Optional[int] = None, is_sorted: bool = False, training: bool = True) -> Tuple[Tensor, Tensor]:
+    """Mirror of torch_geometric.utils.dropout_path (utils/dropout.py:221-298): every edge that a uniform random walk
+    of walk_length steps traverses is dropped, the walks starting walks_per_node times at the source of each edge
+    kept by a Bernoulli(p) draw.  Returns (kept edge_index, edge mask).  The draws are the reference's: the start mask
+    from torch.rand on edge_index's device, then the walks' seed from torch's CPU generator (ops.random_walk)."""
+    if p < 0.0 or p > 1.0:
+        raise ValueError(f"Sample probability has to be between 0 and 1 (got {p}")
+    num_edges = edge_index.size(1)
+    edge_mask = edge_index.new_ones(num_edges, dtype=torch.bool)
+    if not training or p == 0.0:
+        return edge_index, edge_mask
+    if num_nodes is None:
+        num_nodes = int(edge_index.max()) + 1 if edge_index.numel() > 0 else 0
+    if is_sorted:
+        row, col, order = edge_index[0], edge_index[1], None
+    else:
+        row, col, order = sort_edge_index_by_row_col(edge_index, num_nodes)
+    sample_mask = torch.rand(num_edges, device=edge_index.device) <= p
+    start = row[sample_mask].repeat(walks_per_node)
+    walk = ops.random_walk(ops.index2ptr(row.contiguous(), num_nodes), col.contiguous(), start, walk_length)
+    walk_keys = walk[:, :-1].reshape(-1).long() * num_nodes + walk[:, 1:].reshape(-1).long()
+    hit = torch.isin(row.long() * num_nodes + col.long(), walk_keys).nonzero().view(-1)
+    edge_mask[hit if order is None else order[hit]] = False
+    return edge_index[:, edge_mask], edge_mask
+
+
 def add_remaining_self_loops(edge_index: Tensor, edge_attr: Optional[Tensor] = None,
                              fill_value: Optional[float] = None,
                              num_nodes: Optional[int] = None) -> Tuple[Tensor, Optional[Tensor]]:
